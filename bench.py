@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- PAF overlaps/s, ingest -> GFA, on synthetic PAF of the shapes BASELINE.json names.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload NAME] [--impl b200|reference] [--quick]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload NAME] [--impl b200|reference] [--quick] [--dump-outputs DIR]
 
 One "step" = one pass of the whole hot path over one PAF: parse -> read selection -> string graph ->
 transitive reduction -> cleaning -> unitigs (main.c:108-199 of the reference).
@@ -26,6 +26,7 @@ file order (rank r generates and holds part r), read ids are hash-sharded (owner
            reference's time on the same file.
 * host_affinity : every rank runs on the host cores NVML names for its GPU (bound before the pinned buffers are allocated).
 --impl reference prints the same line for the reference's own CPU implementation (rank 0 only).
+--dump-outputs DIR writes the layout the last timed step computed, as a caller of the library receives it, to DIR/<name>.npy.
 """
 import argparse
 import ctypes as C
@@ -37,6 +38,8 @@ import sys
 import tempfile
 import threading
 import time
+
+import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
@@ -110,7 +113,7 @@ def generate(n_reads, seed, name_base=0):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -198,6 +201,46 @@ def reference_full_size(name, shm, model, cores):
     return d
 
 
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(lib, ctx, out_dir):
+    """The read intervals, unitigs and unitig graph the last step left in the context, as mab_export_dict / mab_export_sub /
+    mab_export_ug hand them to a caller (the structs ma_ug_print turns into GFA), one DIR/<name>.npy per field, float64 (every
+    value is an integer below 2^53).  When all of them together pass 64 MB, arrays of equal length keep the same fixed, seeded
+    sample of their rows.  Arrays without rows (a layout whose unitigs have no links, say) are not written."""
+    from miniasm_b200 import capi
+    d, sub, ug = lib.mab_export_dict(ctx), lib.mab_export_sub(ctx), lib.mab_export_ug(ctx)
+    n_seq = d.contents.n_seq
+    s = capi.np_from_ptr(sub, n_seq, capi.SUB_DT)
+    read_len = np.array([d.contents.seq[i].len for i in range(n_seq)])
+    u = ug.contents
+    utg = [u.a[i] for i in range(u.n)]
+    reads = np.concatenate([capi.np_from_ptr(x.a, x.n, np.uint64) for x in utg] + [np.zeros(0, np.uint64)])
+    g = u.g.contents
+    arcs = capi.np_from_ptr(g.arc, g.n_arc_srt & 0x7fffffff, capi.ARC_DT)
+    out = {"read_len": read_len, "read_start": s["s_del"] & 0x7fffffff, "read_end": s["e"], "read_deleted": s["s_del"] >> 31,
+           "utg_len": np.array([x.len_circ & 0x7fffffff for x in utg]), "utg_circular": np.array([x.len_circ >> 31 for x in utg]),
+           "utg_start": np.array([x.start for x in utg]), "utg_end": np.array([x.end for x in utg]), "utg_n_reads": np.array([x.n for x in utg]),
+           "utg_read_vertex": reads >> np.uint64(32), "utg_read_len": reads & np.uint64(0xffffffff),
+           "ug_arc_from": arcs["ul"] >> np.uint64(32), "ug_arc_len": arcs["ul"] & np.uint64(0xffffffff), "ug_arc_to": arcs["v"],
+           "ug_arc_ov": arcs["ol_del"] & 0x7fffffff, "ug_arc_deleted": arcs["ol_del"] >> 31}
+    lib.ma_ug_destroy(ug), capi.c_free(sub), lib.sd_destroy(d)
+    total = sum(len(v) for v in out.values()) * 8
+    keep = {}
+    if total > DUMP_BYTES:
+        for n in sorted({len(v) for v in out.values()}):
+            m = int(n * DUMP_BYTES * 0.95 / total)
+            if m < n:
+                keep[n] = np.sort(np.random.default_rng(n).choice(n, m, replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in out.items():
+        if not len(v):
+            continue
+        v = np.asarray(v, dtype=np.float64)
+        np.save(os.path.join(out_dir, k + ".npy"), v[keep[len(v)]] if len(v) in keep else v)
+
+
 def bind_near_gpu(torch, ordinal):
     """Run this process on the host cores next to its GPU (NVML's CPU affinity of the device), before any pinned buffer exists: the
     buffers then live on that NUMA node and the H2D copies of several ranks do not cross the socket link.  Best effort: any
@@ -251,6 +294,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--quick", action="store_true", help="skip the extra legs: full-size reference run, cold CLI wall clock, noisy workload")
     ap.add_argument("--host-gfa", action="store_true", help="e2e leg: host structs + ma_ug_print instead of the GFA text formatted on the GPU (mab_write_gfa)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed to DIR/<name>.npy (float64)")
     a = ap.parse_args()
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -291,7 +335,7 @@ def main():
         print(json.dumps(line))
         return
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ CUDA arm
     os.environ.setdefault("NCCL_DEBUG", "WARN")
     saved_stdout = os.dup(1)                  # libraries (NCCL banner ...) must not add lines to stdout: the JSON line is the only one
     os.dup2(2, 1)
@@ -330,7 +374,7 @@ def main():
         if world > 1:
             dist.barrier()
 
-    def measure(args_str, steps, warmup, with_roofline):
+    def measure(args_str, steps, warmup, with_roofline, dump_dir=None):
         """value + e2e legs over one PAF (this rank's part of it)."""
         buf, n_bytes, n_lines, free = generate_args(args_str, rank, world)
         pinned = torch.empty(max(n_bytes, 1), dtype=torch.uint8, pin_memory=True)
@@ -385,6 +429,8 @@ def main():
             dt_ms.append((ms, lib.mab_stats(ctx).contents.ms_del_trans_kernel))
         barrier()
         wall_dev = time.perf_counter() - t_wall0
+        if dump_dir and rank == 0:                                 # (the layout is replicated on every rank)
+            dump_outputs(lib, ctx, dump_dir)
         st = lib.mab_stats(ctx).contents
         cl = [C.c_uint32() for _ in range(4)]
         lib.mab_clean_totals(*[C.byref(x) for x in cl])
@@ -432,16 +478,16 @@ def main():
 
     sampler = ClockSampler(local_rank)
     sampler.start()
-    res = measure(wl["args"], a.steps, a.warmup, True)
+    res = measure(wl["args"], a.steps, a.warmup, True, a.dump_outputs)
     clocks = sampler.finish()
     dev_ms, e2e_s, lines_all, bytes_all = reduce_ranks(res)
 
     noisy = None
     if extras:  # the bubble/tip-dense set through the same legs (1 GPU only)
-        nres = measure(WORKLOADS["noisy_600k"]["args"], 3, 1, False)
+        nres = measure(WORKLOADS["noisy_600k"]["args"], a.steps, a.warmup, False)
         noisy = {"workload": WORKLOADS["noisy_600k"]["label"], "pafgen": WORKLOADS["noisy_600k"]["args"], "paf_lines": nres["n_lines"],
-                 "value": nres["n_lines"] * 3 / (nres["dev_ms"] * 1e-3), "ms_per_step": nres["dev_ms"] / 3,
-                 "e2e": {"value": nres["n_lines"] * 3 / nres["e2e_s"], "ms_per_step": nres["e2e_s"] / 3 * 1e3},
+                 "value": nres["n_lines"] * a.steps / (nres["dev_ms"] * 1e-3), "ms_per_step": nres["dev_ms"] / a.steps,
+                 "e2e": {"value": nres["n_lines"] * a.steps / nres["e2e_s"], "ms_per_step": nres["e2e_s"] / a.steps * 1e3},
                  "phase_ms_last_step": nres["phases"], "n_reduced": nres["n_reduced"], "n_utg": nres["n_utg"], "gfa_sha256": nres["gfa_sha256"],
                  "cleaning_passes": nres["cleaning"]}
 
@@ -451,19 +497,11 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except OSError:
             pass
-        peak, peak_src = (peaks["hbm_gbs"], "measured (MEASURED_PEAKS.json, burst copy)") if "hbm_gbs" in peaks else (6650.0, "fallback (B200_PROFILING.md)")
+        peak, peak_src = (peaks["hbm_gbs"], "measured (MEASURED_PEAKS.json, burst copy)") if "hbm_gbs" in peaks else (3350.0, "H100 SXM data sheet (HBM3)")
         n_arc_in, n_vtx, inner, kms = res["n_arc_in"], res["n_vtx"], res["inner"], res["kernel_ms"]
         alg_bytes = 16 * n_arc_in + 16 * inner + 1 * n_arc_in + 12 * n_vtx     # DESIGN.md "roofline": own slab + explored neighbour prefixes + flag byte + idx/seq
         achieved = alg_bytes / (kms * 1e-3) / 1e9 if kms else 0.0
-        traffic = None                             # measured DRAM bytes of one launch: from the committed ncu capture of THIS kernel on THIS workload, 1 GPU only
-        prof = os.path.join(ROOT, "profiles", "del_trans_r02.json")
-        if world == 1 and os.path.exists(prof):
-            try:
-                pj = json.load(open(prof))
-                if pj.get("workload") == name:
-                    traffic = pj.get("dram_bytes_per_launch")
-            except (OSError, ValueError):
-                pass
+        traffic = None                             # measured DRAM bytes of one launch: not measured (no hardware counters here)
         # the other phases against SURVEY.md 8(d): algorithmic bytes / CUDA-event time of the phase (rank 0's share at N > 1)
         n_hits, n_arc_sg, ph = res["n_hits"] // world, res["n_arc_sg"] // world, res["phases"]
         hit_bits = 32 + max(1, (max(res["n_seq"], 2) - 1).bit_length())

@@ -6,7 +6,7 @@
  *     its own driver main.c:108-199 calls.  Every entry point below has the same name, argument meaning,
  *     ownership rules and stderr/exit behaviour as the reference function it replaces, so the reference's
  *     main.o links against this library unchanged (INTEGRATION.md, "link seam").  Arrays are host memory
- *     (malloc/calloc/realloc family); each call moves its operands to the B200, runs the CUDA path and
+ *     (malloc/calloc/realloc family); each call moves its operands to the GPU, runs the CUDA path and
  *     moves the result back.  The struct layouts are ABI: main.c and the writers read fields directly.
  *
  *  2. FUSED level (mab_*).  One opaque device-resident context keeps hits, arcs and the graph in HBM

@@ -1,6 +1,6 @@
 """ctypes view of the miniasm C ABI (include/miniasm_b200.h).
 
-``load_product()`` -> ``miniasm_b200/libminiasm_b200.so`` (CUDA, sm_100a).  ``Lib`` works for any library that exports the
+``load_product()`` -> ``miniasm_b200/libminiasm_b200.so`` (CUDA, sm_90a).  ``Lib`` works for any library that exports the
 reference's C API, which is how the test oracles are driven too -- but their loaders live in ``oracle/loaders.py``, not here.
 """
 import ctypes as C

@@ -1,4 +1,4 @@
-// asg_dev.cu -- string-graph container passes on the GPU (sm_100a).
+// asg_dev.cu -- string-graph container passes on the GPU (sm_90a).
 //
 // Reference behaviour being reproduced (file:line into lh3/miniasm):
 //   asg_arc_rm          asg.c:57-70     stable compaction of live arcs
@@ -38,7 +38,7 @@ __device__ __forceinline__ DArc ld_arc_nc(const DArc *p)
 }
 
 // one LDG.128 through the read-only path, kept as a single instruction even when only some words are used
-// (two 32-bit loads of a 16-byte record cost twice the L1 wavefronts: ncu on k_del_trans_warp v2)
+// (two 32-bit loads of a 16-byte record cost twice the L1 wavefronts)
 __device__ __forceinline__ uint4 ld_arc4(const DArc *p)
 {
 	uint4 t;
@@ -339,8 +339,8 @@ __device__ __forceinline__ uint32_t dt_hash(uint32_t x, uint32_t mask) { return 
 // per slab entry) | hmark (mark per slot: 1 = target of v, 2 = reduced) | slot (table slot of slab entry i) | fmin
 // (lowest slab position per slot, only when a slab holds multi-arcs).  The mark lives in the table, so arcs to the same
 // target share it exactly like mark[] indexed by vertex does in the reference.
-// The kernel is issue-bound (profiles/r01_del_trans.md: the round-1 version spent ~476 warp instructions per vertex,
-// nearly all of them per-vertex bookkeeping), so this version keeps the instruction stream short: peer/no-peer is a
+// The kernel is issue-bound (an earlier version spent ~476 warp instructions per vertex, nearly all of them per-vertex
+// bookkeeping), so this version keeps the instruction stream short: peer/no-peer is a
 // template parameter, the table is cleared with one or two 128-bit stores, every slab loop stays rolled (two entries per
 // lane cover 64 arcs), the next vertex's index/seq words are prefetched, and (SORTED, i.e. whenever the graph says
 // is_srt) a slab sorted by length makes the arcs that satisfy the length bound a prefix by themselves.
@@ -365,8 +365,8 @@ k_del_trans_warp(const DArc *__restrict__ arc, const uint64_t *__restrict__ idx,
 	unsigned long long n_inner = 0;
 
 	// Software pipeline over the vertices of this warp: while vertex v is worked on, the index / seq words of the next one are
-	// already in flight, and its first 64 slab entries are requested as soon as those words have landed -- the ncu source page
-	// of the unpipelined loop had 20 % of all stall samples on the first use of the own slab and 8 % on idx/seq.
+	// already in flight, and its first 64 slab entries are requested as soon as those words have landed: without it the
+	// warps stall on the first use of the own slab and on idx/seq.
 	const uint32_t stride = gridDim.x * DT_WARPS;
 	uint32_t v = blockIdx.x * DT_WARPS + warp;
 	uint64_t iv = 0, iv_n = 0;
@@ -458,7 +458,7 @@ k_del_trans_warp(const DArc *__restrict__ arc, const uint64_t *__restrict__ idx,
 			}
 			// (no __syncwarp here: every lane's reads of hmark feed its ballot predicate and no lane passes the ballot before all have
 			// arrived, so the marks are read before any lane rewrites them below.  racecheck reports the pattern as a warp-level WAR
-			// *warning*; with an explicit barrier it reports nothing and the kernel is 3 % slower -- profiles/r02_racecheck_*.log)
+			// *warning*; an explicit barrier silences it at the cost of a slower kernel)
 			if (nxt >= nv) break;
 			i = nxt;
 			const uint32_t w = hkey[slot[i]], li = tl[i];
@@ -723,7 +723,7 @@ uint32_t dg_del_trans_flags(MabDev &d, DGraph &g, uint32_t fuzz, uint32_t own_lo
 		MAB_CUDA(cudaEventCreate(&e0)); MAB_CUDA(cudaEventCreate(&e1));
 		MAB_CUDA(cudaEventRecord(e0, d.stream));
 		unsigned grid = (n_vtx + DT_WARPS - 1) / DT_WARPS;
-		if (grid > 148u * 64u) grid = 148u * 64u;
+		if (grid > MAB_SMS * 64u) grid = MAB_SMS * 64u;
 		// the inner-iteration counter (for the roofline arithmetic) costs issue slots: only counted when asked for
 		{
 			const bool st = mab_del_trans_count_inner != 0, p2p = peer != nullptr, srt = g.is_srt;
@@ -741,7 +741,7 @@ uint32_t dg_del_trans_flags(MabDev &d, DGraph &g, uint32_t fuzz, uint32_t own_lo
 		if (n_big) {
 			MAB_CUDA(cudaFuncSetAttribute(k_del_trans_cta, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DT_BIG_SMEM)); // per device: set on every use
 			uint32_t *huge = mab_alloc<uint32_t>(d, n_big);
-			MAB_LAUNCH(d, k_del_trans_cta, n_big < 148u * 2 ? n_big : 148u * 2, 256, DT_BIG_SMEM, g.arc, g.idx, fuzz, flag, big, n_big, huge, d.d_scal, sv);
+			MAB_LAUNCH(d, k_del_trans_cta, n_big < MAB_SMS * 2 ? n_big : MAB_SMS * 2, 256, DT_BIG_SMEM, g.arc, g.idx, fuzz, flag, big, n_big, huge, d.d_scal, sv);
 			uint32_t n_huge = (uint32_t)d.get_scal(SC_AUX2);
 			if (n_huge) {
 				uint8_t *mark = mab_alloc<uint8_t>(d, n_vtx);

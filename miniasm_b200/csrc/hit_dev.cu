@@ -59,8 +59,8 @@ void dh_free(MabDev &d, DHits &h)
 }
 
 // ---------------------------------------------------------------------------------------------
-// Stable compaction of hits by a byte flag array.  32-byte records: the generic library selection moves them at
-// ~2.2 TB/s (ncu: 2.8 ms per 100 M hits), so the hit path has its own three-step compaction -- per-tile keep counts
+// Stable compaction of hits by a byte flag array.  32-byte records move well below the copy bandwidth through the
+// generic library selection, so the hit path has its own three-step compaction -- per-tile keep counts
 // (flags only), a scan of the ~n/2048 tile counts, and a scatter in which every warp row reads 1 KB of contiguous
 // records and writes them behind the tile's offset.  Order of the kept hits is the input order.
 // MAB_CUB_SELECT=1 switches back to cub::DeviceSelect::Flagged.
@@ -366,7 +366,7 @@ __device__ __forceinline__ bool sub_hit_keys(const DHit &h, uint32_t qid, float 
 
 // Bitonic network over 32*M keys held in registers, element e = 32*m + lane: exchanges at distance j < 32 are lane
 // shuffles, distances >= 32 pair two registers of the same lane -- no shared-memory traffic and none of the 2-way bank
-// conflicts the strided pair indexing has (ncu: 0.41 G conflicts per launch in the shared-memory version).
+// conflicts the strided pair indexing has in the shared-memory version.
 template <int M>
 __device__ __forceinline__ void warp_bitonic_regs(uint32_t (&v)[M], const int lane)
 {
@@ -450,7 +450,7 @@ k_sub_warp(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, uint32_
 		for (uint32_t i = n + lane; i < np; i += 32) key[i] = 0xffffffffu;
 		__syncwarp();
 		// bitonic network; j = 1 << lj is a power of two, so the pair index comes from shifts (a 32-bit division per
-		// compare-exchange made this loop ~90 % of the kernel's instructions: ncu, profiles/r01_launches_c3_summary.txt)
+		// compare-exchange made this loop most of the kernel's instructions)
 		for (uint32_t k = 2, lk = 1; k <= np; k <<= 1, ++lk)
 			for (uint32_t lj = lk; lj-- > 0;) {
 				const uint32_t j = 1u << lj;
@@ -634,7 +634,7 @@ uint64_t dh_sub(MabDev &d, const DHits &h, int min_dp, float min_iden, int end_c
 	MAB_CUDA(cudaMemsetAsync(d.d_scal, 0, 8 * sizeof(unsigned long long), d.stream));
 	MAB_LAUNCH(d, k_group_bounds, mab_grid(h.n, 256), 256, 0, h.a, h.n, (uint32_t*)grp);
 	unsigned grid = (n_seq + SUBW_WARPS - 1) / SUBW_WARPS;
-	if (grid > 148u * 32u) grid = 148u * 32u;
+	if (grid > MAB_SMS * 32u) grid = MAB_SMS * 32u;
 	static const int smem_sort = getenv("MAB_SUB_SMEM_SORT") && atoi(getenv("MAB_SUB_SMEM_SORT")) != 0; // 1: the shared-memory network
 	MAB_LAUNCH(d, k_sub_warp, grid, SUBW_WARPS * 32, 0, h.a, grp, n_seq, min_dp, min_iden, (uint32_t)end_clip, sub_out, big, d.d_scal, smem_sort);
 	uint32_t n_big = (uint32_t)d.get_scal(SC_BIG);
@@ -642,7 +642,7 @@ uint64_t dh_sub(MabDev &d, const DHits &h, int min_dp, float min_iden, int end_c
 		const size_t smem = (size_t)SUBC_HITS * 2 * 4;
 		MAB_CUDA(cudaFuncSetAttribute(k_sub_cta, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); // per device: set on every use
 		uint32_t *huge = mab_alloc<uint32_t>(d, n_big);
-		MAB_LAUNCH(d, k_sub_cta, n_big < 148u * 2 ? n_big : 148u * 2, 512, smem, h.a, grp, big, n_big, min_dp, min_iden, (uint32_t)end_clip, sub_out, huge, d.d_scal);
+		MAB_LAUNCH(d, k_sub_cta, n_big < MAB_SMS * 2 ? n_big : MAB_SMS * 2, 512, smem, h.a, grp, big, n_big, min_dp, min_iden, (uint32_t)end_clip, sub_out, huge, d.d_scal);
 		uint32_t n_huge = (uint32_t)d.get_scal(SC_AUX2);
 		if (n_huge) { // reads with more hits than a CTA can sort: device-wide sort of everything, keep only their rows
 			DSub *tmp = mab_alloc<DSub>(d, n_seq);
@@ -1194,13 +1194,13 @@ static bool sg_emit_segmented(MabDev &d, const DHits &h, const HitArcParams &p, 
 		++d.n_lib;
 		dg_reserve(d, g, n_arc ? n_arc : 1);
 		unsigned grid = (n_seq + SGW_WARPS - 1) / SGW_WARPS;
-		if (grid > 148u * 32u) grid = 148u * 32u;
+		if (grid > MAB_SMS * 32u) grid = MAB_SMS * 32u;
 		MAB_LAUNCH(d, k_sg_sort_warp, grid, SGW_WARPS * 32, 0, h.a, grp, epos, g.seq, n_seq, p, lb, g.arc, big, d.d_scal);
 		const uint32_t n_big = (uint32_t)d.get_scal(SC_BIG);
 		if (n_big) {
 				const size_t smem = (size_t)SGC_HITS * 16;
 			MAB_CUDA(cudaFuncSetAttribute(k_sg_sort_cta, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-			MAB_LAUNCH(d, k_sg_sort_cta, n_big < 148u ? n_big : 148u, 512, smem, h.a, grp, epos, g.seq, big, n_big, p, g.arc, d.d_scal);
+			MAB_LAUNCH(d, k_sg_sort_cta, n_big < MAB_SMS ? n_big : MAB_SMS, 512, smem, h.a, grp, epos, g.seq, big, n_big, p, g.arc, d.d_scal);
 			if (d.get_scal(SC_AUX) != 0) ok = false; // a read with more hits than a CTA sorts
 		}
 	}

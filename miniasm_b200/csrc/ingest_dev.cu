@@ -200,9 +200,9 @@ __host__ __device__ __forceinline__ uint32_t num_field(const char *p, uint32_t s
 
 // Parse one line [p, e) (no terminator, '\r' already dropped), one thread per line.
 // Pass 1 finds the first 11 TABs a 32-bit word at a time (SWAR compare, positions parked in shared memory);
-// pass 2 converts each column from its known byte range.  The earlier byte-at-a-time loops cost ~170 warp
-// instructions per line because the 32 lines of a warp sit in different columns at every step (ncu: 8.5 G
-// instructions, 10 ms at 50 M lines); with the boundaries known up front the per-column loops are short and uniform.
+// pass 2 converts each column from its known byte range.  Byte-at-a-time loops cost ~170 warp instructions per line
+// because the 32 lines of a warp sit in different columns at every step; with the boundaries known up front the
+// per-column loops are short and uniform.
 // Semantics: columns split on TAB only; numbers follow strtol(.,10) truncated to 32 bits (ml to 31); rev = first
 // byte of column 5 is '-'.  tab: this lane's column of an [11][32] shared scratch.
 __host__ __device__ __forceinline__ void parse_line(const char *p, const char *e, PLine &r, uint32_t *tab)
@@ -294,7 +294,7 @@ __device__ __forceinline__ uint32_t tab_insert(const NameTab &t, const char *__r
 
 // One CTA parses PARSE_LINES consecutive lines.  Their bytes are contiguous in the file, so the CTA first copies
 // the whole range into shared memory with coalesced 128-bit loads and the threads then walk their own line there:
-// byte-wise walking of global memory made every warp-level load touch ~16 cache lines (ncu: L1 wavefront bound).
+// byte-wise walking of global memory makes every warp-level load touch ~16 cache lines (L1 wavefront bound).
 // A range that does not fit (very long lines) is parsed straight from global memory.
 // Fused into the same pass (round 1 ran them as three more sweeps over a 64-byte record): the store filter of
 // hit.c:85 and the dictionary insert of both names, while the line is still in shared memory.
@@ -483,7 +483,7 @@ uint64_t *dev_line_starts(MabDev &d, const char *d_text, size_t len, uint64_t *n
 	const uint64_t n_tile = (len + NL_TILE - 1) / NL_TILE;
 	uint64_t *cnt = mab_alloc<uint64_t>(d, n_tile + 1);
 	uint64_t *base = mab_alloc<uint64_t>(d, n_tile + 1);
-	MAB_LAUNCH(d, k_nl_count, mab_grid(n_tile, 1, 148u * 32u), NL_THREADS, 0, d_text, len, n_tile, cnt);
+	MAB_LAUNCH(d, k_nl_count, mab_grid(n_tile, 1, MAB_SMS * 32u), NL_THREADS, 0, d_text, len, n_tile, cnt);
 	size_t tb = 0;
 	cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt, base, (int64_t)(n_tile + 1), d.stream);
 	void *tmp = d.tmp(tb);
@@ -495,7 +495,7 @@ uint64_t *dev_line_starts(MabDev &d, const char *d_text, size_t len, uint64_t *n
 	const uint64_t n_lines = n_nl + 1; // newlines that are followed by at least one byte, plus the first line
 	uint64_t *start = mab_alloc<uint64_t>(d, n_lines + 1);
 	MAB_CUDA(cudaMemsetAsync(start, 0, 8, d.stream));
-	MAB_LAUNCH(d, k_nl_write, mab_grid(n_tile, 1, 148u * 32u), NL_THREADS, 0, d_text, len, n_tile, base, start + 1);
+	MAB_LAUNCH(d, k_nl_write, mab_grid(n_tile, 1, MAB_SMS * 32u), NL_THREADS, 0, d_text, len, n_tile, base, start + 1);
 	d.free(cnt); d.free(base);
 	*n_lines_out = n_lines;
 	return start;
@@ -557,7 +557,7 @@ void ingest_paf(MabDev &d, const char *d_text, size_t len, int min_span, int min
 		tab = tab_alloc(d, cap);
 		d.zero_scal(SC_COUNT, 4);
 		set_rng(d, 0, n_lines, n_lines);
-		MAB_LAUNCH(d, k_parse, mab_grid((n_lines + PARSE_LINES - 1) / PARSE_LINES, 1, 148u * 16u), PARSE_LINES, 0, d_text, len, start, d.d_scal + SC_RNG, min_span, min_match, tab, ln, d.d_scal + SC_COUNT);
+		MAB_LAUNCH(d, k_parse, mab_grid((n_lines + PARSE_LINES - 1) / PARSE_LINES, 1, MAB_SMS * 16u), PARSE_LINES, 0, d_text, len, start, d.d_scal + SC_RNG, min_span, min_match, tab, ln, d.d_scal + SC_COUNT);
 		st.n_parsed = d.get_scal(SC_COUNT);
 		if (d.h_scal[SC_COUNT + 2] == 0) break;
 		d.free(tab.key); d.free(tab.first); d.free(tab.id);
@@ -607,12 +607,12 @@ static bool stream_parse(MabDev &d, char *d_text, const char *host_text, size_t 
 		MAB_CUDA(cudaMemcpyAsync(d_text + b0, host_text + b0, b1 - b0, cudaMemcpyHostToDevice, d.copy_stream));
 		MAB_CUDA(cudaEventRecord(ev[k], d.copy_stream));
 		MAB_CUDA(cudaStreamWaitEvent(d.stream, ev[k], 0));
-		MAB_LAUNCH(d, k_nl_count_range, mab_grid(t1 - t0, 1, 148u * 8u), NL_THREADS, 0, d_text, len, t0, t1, cnt);
+		MAB_LAUNCH(d, k_nl_count_range, mab_grid(t1 - t0, 1, MAB_SMS * 8u), NL_THREADS, 0, d_text, len, t0, t1, cnt);
 		cub::DeviceScan::ExclusiveSum(tmp, tb, cnt, base, (int64_t)(t1 - t0), d.stream);
 		++d.n_lib;
-		MAB_LAUNCH(d, k_nl_write_range, mab_grid(t1 - t0, 1, 148u * 8u), NL_THREADS, 0, d_text, len, t0, t1, base, state, start);
+		MAB_LAUNCH(d, k_nl_write_range, mab_grid(t1 - t0, 1, MAB_SMS * 8u), NL_THREADS, 0, d_text, len, t0, t1, base, state, start);
 		MAB_LAUNCH(d, k_nl_advance, 1, 32, 0, state, base, cnt, t1 - t0, state + 4, (int)(k + 1 == n_chunk));
-		MAB_LAUNCH(d, k_parse, 148u * 8u, PARSE_LINES, 0, d_text, len, start, state + 4, min_span, min_match, tab, ln, d.d_scal + SC_COUNT);
+		MAB_LAUNCH(d, k_parse, MAB_SMS * 8u, PARSE_LINES, 0, d_text, len, start, state + 4, min_span, min_match, tab, ln, d.d_scal + SC_COUNT);
 	}
 	unsigned long long fin[8];
 	MAB_CUDA(cudaMemcpyAsync(fin, state, sizeof(fin), cudaMemcpyDeviceToHost, d.stream));
@@ -1043,7 +1043,7 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 			tab = tab_alloc(d, cap);
 			d.zero_scal(SC_COUNT, 4);
 			set_rng(d, 0, n_lines, n_lines);
-			if (n_lines) MAB_LAUNCH(d, k_parse, mab_grid((n_lines + PARSE_LINES - 1) / PARSE_LINES, 1, 148u * 16u), PARSE_LINES, 0, d_text, len, start, d.d_scal + SC_RNG, min_span, min_match, tab, ln, d.d_scal + SC_COUNT);
+			if (n_lines) MAB_LAUNCH(d, k_parse, mab_grid((n_lines + PARSE_LINES - 1) / PARSE_LINES, 1, MAB_SMS * 16u), PARSE_LINES, 0, d_text, len, start, d.d_scal + SC_RNG, min_span, min_match, tab, ln, d.d_scal + SC_COUNT);
 			n_parsed = d.get_scal(SC_COUNT);
 			overflow = d.h_scal[SC_COUNT + 2] != 0;
 		}
@@ -1225,7 +1225,7 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 	uint32_t *blk_cnt = mab_alloc<uint32_t>(d, (size_t)G * n_blk + 1);
 	uint64_t *blk_off = mab_alloc<uint64_t>(d, (size_t)G * n_blk + 1);
 	MAB_CUDA(cudaMemsetAsync(blk_cnt, 0, ((size_t)G * n_blk + 1) * 4, d.stream));
-	if (n_blk) MAB_LAUNCH(d, k_push_count, mab_grid(n_blk, 1, 148u * 8u), PUSH_LINES, 0, ln, n_lines, tab, bi_dir, (uint32_t)G, n_blk, blk_cnt);
+	if (n_blk) MAB_LAUNCH(d, k_push_count, mab_grid(n_blk, 1, MAB_SMS * 8u), PUSH_LINES, 0, ln, n_lines, tab, bi_dir, (uint32_t)G, n_blk, blk_cnt);
 	{
 		cub::TransformInputIterator<uint64_t, U32ToU64i, const uint32_t*> in(blk_cnt, U32ToU64i());
 		size_t tb = 0;
@@ -1258,7 +1258,7 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 		MAB_CUDA(cudaMemcpyAsync(d_pos, pos_base.data(), sizeof(long long) * (size_t)G, cudaMemcpyHostToDevice, d.stream));
 		MAB_CUDA(cudaMemcpyAsync(d_dst, peer.data(), sizeof(void*) * (size_t)G, cudaMemcpyHostToDevice, d.stream));
 		d.zero_scal(SC_AUX, 1);
-		if (n_blk) MAB_LAUNCH(d, k_push_emit, mab_grid(n_blk, 1, 148u * 8u), PUSH_LINES, 0, ln, n_lines, tab, bi_dir, carry, (uint32_t)G, n_blk, blk_off, d_pos, d_dst, (unsigned*)(d.d_scal + SC_AUX));
+		if (n_blk) MAB_LAUNCH(d, k_push_emit, mab_grid(n_blk, 1, MAB_SMS * 8u), PUSH_LINES, 0, ln, n_lines, tab, bi_dir, carry, (uint32_t)G, n_blk, blk_off, d_pos, d_dst, (unsigned*)(d.d_scal + SC_AUX));
 		max_qs = (uint32_t)(d.get_scal(SC_AUX) & 0xffffffffu);
 		{ // nobody sorts before everybody has finished writing: a one-word all-reduce, stream-ordered after the emit kernel on every rank
 			std::vector<uint64_t> mq = sc_allgather_u64(d, sc, max_qs);

@@ -96,9 +96,12 @@ struct MabDev {
 	double trace_t = 0;
 };
 
+// Streaming multiprocessors of the H100 SXM: the grid caps of the grid-stride kernels are multiples of it.
+constexpr unsigned MAB_SMS = 132u;
+
 template <typename T> static inline T *mab_alloc(MabDev &d, size_t n) { return (T*)d.alloc((n ? n : 1) * sizeof(T)); }
 
-static inline unsigned mab_grid(size_t n, unsigned block, unsigned max_blocks = 148u * 32u)
+static inline unsigned mab_grid(size_t n, unsigned block, unsigned max_blocks = MAB_SMS * 32u)
 {
 	size_t g = (n + block - 1) / block;
 	if (g < 1) g = 1;

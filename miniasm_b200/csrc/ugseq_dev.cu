@@ -231,7 +231,7 @@ int dg_ugseq_fill(MabDev &d, const char *text, size_t len, const DReadsIndex &ix
 	MAB_LAUNCH(d, k_rtab_insert, mab_grid(n_seq, 256), 256, 0, n_seq, orig, noff, nlen, ntext, t, d.d_scal + SC_TMP0);
 	MAB_LAUNCH(d, k_rec_lookup, mab_grid(ix.n_rec, 256), 256, 0, ix.n_rec, ix.hdr_line, text, len, ix.start, ix.n_lines, t, orig, noff, nlen, ntext, rec_of_read);
 	SeqSrc f{text, ix.start, ix.type, ix.slen, ix.cum, ix.hdr_line, ix.n_rec, ix.n_lines, ix.fq4};
-	const uint64_t n_warp = ug.n_items < 148ull * 64 ? ug.n_items : 148ull * 64;
+	const uint64_t n_warp = ug.n_items < (uint64_t)MAB_SMS * 64 ? ug.n_items : (uint64_t)MAB_SMS * 64;
 	MAB_LAUNCH(d, k_ugseq_gather, (unsigned)((n_warp * 32 + 255) / 256), 256, 0, f, ug.meta, ug.n_utg, ug.items, ioff, ug.n_items, rec_of_read, sub, seq_pos, out, d.d_scal + SC_TMP0 + 1);
 	const uint64_t overflow = d.get_scal(SC_TMP0), n_short = d.h_scal[SC_TMP0 + 1];
 	d.free(t.key); d.free(t.id); d.free(rec_of_read);

@@ -2,7 +2,7 @@
  * loads or calls this file; only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline leg may.
  *
  * A sequential CPU restatement, in plain C, of the PAF -> string graph -> unitig path of lh3/miniasm
- * v0.3-r179, written from the behaviour of the reference (citations are file:line into /root/reference).
+ * v0.3-r179, written from the behaviour of the reference (citations are file:line into the reference's sources).
  * It exports the reference's own C API names, so the same ctypes driver (miniasm_b200/pipeline.py) can run
  * the reference, this port and the CUDA product side by side.
  *

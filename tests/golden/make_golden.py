@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Regenerates tests/golden/*.json (+ small .gfa.gz) by running the UNMODIFIED reference binary
-(oracle/_ref/miniasm_ref, built from /root/reference by oracle/Makefile) on deterministic synthetic PAFs.
+(oracle/_ref/miniasm_ref, built from the reference's sources by oracle/Makefile) on deterministic synthetic PAFs.
 
 The reference ships no tests or vectors of its own, so these files are the pinned known answers for the
 CPU-only test tier: final GFA and the `-S k -p paf|sg|bed|ug` stage dumps the reference offers as debug

@@ -1,5 +1,6 @@
 """GPU parity of the string-graph container passes (SURVEY.md 8a rows a12-a18) against the
-unmodified reference, function by function through the C ABI, on graphs the reference itself built."""
+unmodified reference, function by function through the C ABI, on graphs the oracle port built (the reference's results
+for the same pre-states are stored digests, tests/refgold.py)."""
 import ctypes as C
 
 import numpy as np
@@ -16,12 +17,12 @@ SETS = ["tiny_exact", "small_exact", "jitter30", "varlen300", "bubbles800", "cha
 
 
 @pytest.fixture(scope="module")
-def graphs(ref, paf_dir):
-    """name -> reference pipeline stopped right after ma_sg_gen (sorted + indexed raw graph)."""
+def graphs(port, paf_dir):
+    """name -> port pipeline stopped right after ma_sg_gen (sorted + indexed raw graph)."""
     out = {}
     for name in SETS:
         paf = synth.generate(name, f"{paf_dir}/{name}.paf")
-        out[name] = Pipeline(ref, paf).read().select().sg_gen()
+        out[name] = Pipeline(port, paf).read().select().sg_gen()
     yield out
     for p in out.values():
         p.free()
@@ -35,115 +36,122 @@ def _clone_to(lib, src_lib, g):
     return h
 
 
-def _same_graph(prod, gp, ref, gr, exact_order=True):
-    ap, sp, ip, srt_p, symm_p = prod.read_graph(gp)
-    ar, sr, ir, srt_r, symm_r = ref.read_graph(gr)
-    assert len(ap) == len(ar)
-    assert np.array_equal(sp, sr)
-    assert (srt_p, symm_p) == (srt_r, symm_r)
-    if exact_order:
-        assert np.array_equal(ap, ar)
-    else:
-        assert np.array_equal(ap["ul"], ar["ul"])          # same sort keys position by position
-        assert np.array_equal(canon_arcs(ap), canon_arcs(ar))
-    assert (ip is None) == (ir is None)
-    if ip is not None:
-        assert np.array_equal(ip, ir)
+def _state(lib, g, exact_order=True):
+    """What the comparison of two graphs looks at; with exact_order=False the arcs are compared by their sort keys position by
+    position and as a canonical multiset (the reference's radix sort is unstable: ties may permute)."""
+    a, s, i, srt, symm = lib.read_graph(g)
+    arcs = [a] if exact_order else [a["ul"], canon_arcs(a)]
+    return [len(a), s, srt, symm, *arcs, i]
+
+
+def _run(lib, src_lib, g, fn, *args, exact_order=True):
+    """fn(lib, clone of g) -> (its return value, state of the clone afterwards)."""
+    h = _clone_to(lib, src_lib, g)
+    n = fn(lib, h, *args)
+    out = (n, _state(lib, h, exact_order))
+    lib.asg_destroy(h)
+    return out
+
+
+def _del_trans(lib, g, fuzz):
+    return lib.asg_arc_del_trans(g, fuzz)
 
 
 @pytest.mark.parametrize("name", SETS)
-def test_del_trans(name, graphs, ref, prod):
+def test_del_trans(name, graphs, port, ref, prod, gold):
     p = graphs[name]
-    gr, gp = _clone_to(ref, ref, p.sg), _clone_to(prod, ref, p.sg)
-    nr = ref.asg_arc_del_trans(gr, p.opt.gap_fuzz)
-    n_p = prod.asg_arc_del_trans(gp, p.opt.gap_fuzz)
-    assert n_p == nr
-    _same_graph(prod, gp, ref, gr)
-    ref.asg_destroy(gr), prod.asg_destroy(gp)
+    gold.expect(_run(prod, port, p.sg, _del_trans, p.opt.gap_fuzz), lambda: _run(ref, port, p.sg, _del_trans, p.opt.gap_fuzz))
 
 
 @pytest.mark.parametrize("fuzz", [0, 10, 100000])
-def test_del_trans_fuzz(fuzz, graphs, ref, prod):
+def test_del_trans_fuzz(fuzz, graphs, port, ref, prod, gold):
     p = graphs["chaos"]
-    gr, gp = _clone_to(ref, ref, p.sg), _clone_to(prod, ref, p.sg)
-    assert prod.asg_arc_del_trans(gp, fuzz) == ref.asg_arc_del_trans(gr, fuzz)
-    _same_graph(prod, gp, ref, gr)
-    ref.asg_destroy(gr), prod.asg_destroy(gp)
+    gold.expect(_run(prod, port, p.sg, _del_trans, fuzz), lambda: _run(ref, port, p.sg, _del_trans, fuzz))
 
 
-def test_del_trans_deleted_reads(graphs, ref, prod):
+def _graph_with_idx(lib, arcs, seq, idx):
+    g = lib.make_graph(arcs, seq, True)
+    g.contents.idx = capi.c_malloc_copy(idx)
+    return g
+
+
+def test_del_trans_deleted_reads(graphs, port, ref, prod, gold):
     """reads flagged del lose every arc (asg.c:158-161)."""
     p = graphs["jitter30"]
-    arcs, seq, idx, _, _ = ref.read_graph(p.sg)
+    arcs, seq, idx, _, _ = port.read_graph(p.sg)
     seq = seq.copy()
     seq[::7] |= DEL
-    gr, gp = ref.make_graph(arcs, seq, True), prod.make_graph(arcs, seq, True)
-    gr.contents.idx, gp.contents.idx = capi.c_malloc_copy(idx), capi.c_malloc_copy(idx)
-    assert prod.asg_arc_del_trans(gp, 1000) == ref.asg_arc_del_trans(gr, 1000)
-    _same_graph(prod, gp, ref, gr)
-    ref.asg_destroy(gr), prod.asg_destroy(gp)
+    g = _graph_with_idx(port, arcs, seq, idx)
+    gold.expect(_run(prod, port, g, _del_trans, 1000), lambda: _run(ref, port, g, _del_trans, 1000))
+    port.asg_destroy(g)
 
 
 @pytest.mark.parametrize("w2_first", [False, True])
-def test_del_trans_tied_arcs(w2_first, ref, prod):
+def test_del_trans_tied_arcs(w2_first, port, ref, prod, gold):
     """Two arcs tied on (source, length) whose targets overlap each other (tests/tied_graph.py): for either slab order the kernel
     reduces what the reference's sequential walk reduces -- the counter differs between the two orders, never between the two sides."""
-    arcs, seq, idx = tied_graph(w2_first)
-    gr, gp = ref.make_graph(arcs, seq, True), prod.make_graph(arcs, seq, True)
-    gr.contents.idx, gp.contents.idx = capi.c_malloc_copy(idx), capi.c_malloc_copy(idx)
-    nr = ref.asg_arc_del_trans(gr, FUZZ)
-    assert prod.asg_arc_del_trans(gp, FUZZ) == nr
-    assert nr == (4 if w2_first else 3)                        # v -> x is reduced by the pass itself only when w2 is walked first
-    _same_graph(prod, gp, ref, gr)
-    ref.asg_destroy(gr), prod.asg_destroy(gp)
+    g = _graph_with_idx(port, *tied_graph(w2_first))
+    got = _run(prod, port, g, _del_trans, FUZZ)
+    assert got[0] == (4 if w2_first else 3)                    # v -> x is reduced by the pass itself only when w2 is walked first
+    gold.expect(got, lambda: _run(ref, port, g, _del_trans, FUZZ))
+    port.asg_destroy(g)
+
+
+def _cleanup(lib, g):
+    lib.asg_cleanup(g)
 
 
 @pytest.mark.parametrize("name", ["small_exact", "chaos", "skew_small"])
-def test_cleanup_sorts_and_indexes(name, graphs, ref, prod):
+def test_cleanup_sorts_and_indexes(name, graphs, port, ref, prod, gold):
     """asg_cleanup on a shuffled, partly deleted arc set: rm + sort + index (asg.c:57-80)."""
     p = graphs[name]
-    arcs, seq, _, _, _ = ref.read_graph(p.sg)
+    arcs, seq, _, _, _ = port.read_graph(p.sg)
     rng = np.random.default_rng(7)
     arcs = arcs[rng.permutation(len(arcs))].copy()
     arcs["ol_del"][rng.random(len(arcs)) < 0.1] |= DEL
     seq = seq.copy()
     seq[rng.random(len(seq)) < 0.02] |= DEL
-    gr, gp = ref.make_graph(arcs, seq), prod.make_graph(arcs, seq)
-    ref.asg_cleanup(gr), prod.asg_cleanup(gp)
-    _same_graph(prod, gp, ref, gr, exact_order=False)   # the reference's radix sort is unstable: ties may permute
-    a = prod.read_graph(gp)[0]
-    assert np.all(a["ul"][1:] >= a["ul"][:-1])
-    ref.asg_destroy(gr), prod.asg_destroy(gp)
+    g = port.make_graph(arcs, seq)
+    got = _run(prod, port, g, _cleanup, exact_order=False)   # the reference's radix sort is unstable: ties may permute
+    gold.expect(got, lambda: _run(ref, port, g, _cleanup, exact_order=False))
+    ul = got[1][4]
+    assert np.all(ul[1:] >= ul[:-1])
+    port.asg_destroy(g)
+
+
+def _cleanup_symm(lib, g):
+    lib.asg_cleanup(g)
+    lib.asg_symm(g)
 
 
 @pytest.mark.parametrize("name", ["chaos", "bubbles800", "skew_small"])
-def test_symm(name, graphs, ref, prod):
+def test_symm(name, graphs, port, ref, prod, gold):
     """asg_symm = del_multi + del_asymm (asg.c:104-145) on a graph with planted duplicates / one-sided arcs."""
     p = graphs[name]
-    arcs, seq, _, _, _ = ref.read_graph(p.sg)
+    arcs, seq, _, _, _ = port.read_graph(p.sg)
     rng = np.random.default_rng(11)
     dup = arcs[rng.random(len(arcs)) < 0.01].copy()
     dup["ul"] += 3                                          # same source + target, longer: a multi-arc
     arcs = np.concatenate([arcs[rng.random(len(arcs)) > 0.01], dup])
-    gr, gp = ref.make_graph(arcs, seq), prod.make_graph(arcs, seq)
-    ref.asg_cleanup(gr), prod.asg_cleanup(gp)
-    ref.asg_symm(gr), prod.asg_symm(gp)
-    _same_graph(prod, gp, ref, gr, exact_order=False)
-    ref.asg_destroy(gr), prod.asg_destroy(gp)
+    g = port.make_graph(arcs, seq)
+    gold.expect(_run(prod, port, g, _cleanup_symm, exact_order=False), lambda: _run(ref, port, g, _cleanup_symm, exact_order=False))
+    port.asg_destroy(g)
+
+
+def _del_short(lib, g, ratio):
+    return lib.asg_arc_del_short(g, ratio)
 
 
 @pytest.mark.parametrize("ratio", [0.5, 0.6, 0.7, 0.8, 0.95])
-def test_del_short(ratio, graphs, ref, prod):
+def test_del_short(ratio, graphs, port, ref, prod, gold):
     p = graphs["chaos"]
-    gr = _clone_to(ref, ref, p.sg)
-    ref.asg_arc_del_trans(gr, 1000)
-    gp = _clone_to(prod, ref, gr)
-    assert prod.asg_arc_del_short(gp, ratio) == ref.asg_arc_del_short(gr, ratio)
-    _same_graph(prod, gp, ref, gr)
-    ref.asg_destroy(gr), prod.asg_destroy(gp)
+    g = port.clone_graph(p.sg)
+    port.asg_arc_del_trans(g, 1000)
+    gold.expect(_run(prod, port, g, _del_short, ratio), lambda: _run(ref, port, g, _del_short, ratio))
+    port.asg_destroy(g)
 
 
-def test_big_slabs(ref, prod):
+def test_big_slabs(port, ref, prod, gold):
     """A hub vertex beyond the warp kernel (128 arcs) and beyond the CTA kernel (8192 arcs)."""
     rng = np.random.default_rng(5)
     n_seq = 12000
@@ -160,15 +168,13 @@ def test_big_slabs(ref, prod):
         for k in range(0, deg - 1, 3):                      # chain some targets so that reductions happen
             add(int(tg[k]), int(tg[k + 1]), int(max(1, ls[k + 1] - ls[k])))
     arcs = np.array(rows, dtype=ARC_DT)
-    gr = ref.make_graph(arcs, seq)
-    ref.asg_cleanup(gr)
-    gp = _clone_to(prod, ref, gr)      # same slab order on both sides: lengths tie heavily here (DESIGN.md "tie order")
-    assert prod.asg_arc_del_trans(gp, 1000) == ref.asg_arc_del_trans(gr, 1000)
-    _same_graph(prod, gp, ref, gr)
-    ref.asg_destroy(gr), prod.asg_destroy(gp)
+    g = port.make_graph(arcs, seq)
+    port.asg_cleanup(g)                # same slab order on both sides: lengths tie heavily here (DESIGN.md "tie order")
+    gold.expect(_run(prod, port, g, _del_trans, 1000), lambda: _run(ref, port, g, _del_trans, 1000))
+    port.asg_destroy(g)
 
 
-def test_empty_graph(ref, prod):
+def test_empty_graph(prod):
     seq = np.full(10, 5000, dtype=np.uint32)
     gp = prod.make_graph(np.zeros(0, dtype=ARC_DT), seq)
     prod.asg_cleanup(gp)

@@ -258,7 +258,7 @@ def _model_worker(rank, world, port, paf, q):
 def test_sharding_scheme_model(world, built, paf_dir):
     from oracle import loaders
     if not os.path.exists(loaders.REFERENCE_SO):
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
+        pytest.skip("oracle/_ref not built (needs the reference's sources)")
     paf = synth.generate("-n 3000 -s 78 -j 300 -l 8000 -L 12000", f"{paf_dir}/dist_model.paf")
     ctx = mp.get_context("spawn")
     q = ctx.Queue()

@@ -1,5 +1,6 @@
 """GPU parity of stage (i) (SURVEY.md 8a rows a4-a11): every drop-in entry point of hit.c / ma_sg_gen is run
-on the state the unmodified reference produced for the previous step and compared bit for bit."""
+on the state the oracle port produced for the previous step and compared bit for bit with what the unmodified reference
+gives from that state (stored digests, tests/refgold.py)."""
 import ctypes as C
 
 import numpy as np
@@ -31,62 +32,56 @@ def pafs(paf_dir):
     return {name: synth.generate(name, f"{paf_dir}/{name}.paf") for name in SETS}
 
 
+def _read_state(p):
+    """ma_hit_read: ids/names, lengths, key order (ties may permute: unstable reference sort) and the multiset of hits."""
+    h = p.hits_np()
+    return [p.names(), p.seq_lens(), h["qns"], canon_hits(h)]
+
+
+def _hits_state(p):
+    return [p.n_hits, canon_mask(p.hits_np())]
+
+
+def _graph_state(p):
+    a, s, i, srt, _ = p.graph_np()
+    return [srt, s, i, a["ul"], canon_arcs(a)]
+
+
+# step -> what is compared after it (from the same pre-state on both sides)
+STEPS = [("sub1", lambda p: [p.sub_np()]), ("cut", _hits_state), ("flt", lambda p: _hits_state(p) + [p.cov.value]),
+         ("sub2_cut_merge", lambda p: [p.sub_np()] + _hits_state(p)), ("contained", lambda p: [p.names(), p.sub_np()] + _hits_state(p)),
+         ("sg_gen", _graph_state)]
+
+
 @pytest.mark.parametrize("name", SETS)
-def test_stage_i_stepwise(name, pafs, ref, prod):
-    r = Pipeline(ref, pafs[name]).read()
+def test_stage_i_stepwise(name, pafs, port, ref, prod, gold):
     p = Pipeline(prod, pafs[name]).read()
-    # ma_hit_read: same ids/names, same multiset of hits, same key order (ties may permute: unstable reference sort)
-    assert r.names() == p.names() and np.array_equal(r.seq_lens(), p.seq_lens())
-    hr, hp = r.hits_np(), p.hits_np()
-    assert len(hr) == len(hp) and np.array_equal(hr["qns"], hp["qns"])
-    assert np.array_equal(canon_hits(hr), canon_hits(hp))
+    gold.expect(_read_state(p), lambda: _read_state(Pipeline(ref, pafs[name]).read()))
+    p.free()
+    r = Pipeline(port, pafs[name]).read()                      # the pre-state of every step: the port's pipeline
 
-    def fresh():
-        return Pipeline(prod, pafs[name], opt=r.opt).adopt(r)
+    def after(lib, step, state):
+        q = Pipeline(lib, pafs[name], opt=r.opt).adopt(r)
+        getattr(q, step)()
+        out = state(q)
+        q.free()
+        return out
 
-    def same_hits(x, y):
-        return x.n_hits == y.n_hits and np.array_equal(canon_mask(x.hits_np()), canon_mask(y.hits_np()))
-
-    # ma_hit_sub (round 1)
-    q = fresh()
-    r.sub1(), q.sub1()
-    assert np.array_equal(r.sub_np(), q.sub_np())
-    q.free()
-    # ma_hit_cut
-    q = fresh()
-    r.cut(), q.cut()
-    assert same_hits(r, q)
-    q.free()
-    # ma_hit_flt
-    q = fresh()
-    r.flt(), q.flt()
-    assert same_hits(r, q)
-    assert r.cov.value == q.cov.value or (np.isnan(r.cov.value) and np.isnan(q.cov.value))
-    q.free()
-    # ma_hit_sub (round 2, end clip) + ma_hit_cut + ma_sub_merge
-    q = fresh()
-    r.sub2_cut_merge(), q.sub2_cut_merge()
-    assert np.array_equal(r.sub_np(), q.sub_np())
-    assert same_hits(r, q)
-    q.free()
-    # ma_hit_contained (+ dictionary squeeze)
-    q = fresh()
-    r.contained(), q.contained()
-    assert r.names() == q.names()
-    assert np.array_equal(r.sub_np(), q.sub_np())
-    assert same_hits(r, q)
-    q.free()
-    # ma_sg_gen
-    q = fresh()
-    r.sg_gen(), q.sg_gen()
-    ar, sr, ir, _, _ = r.graph_np()
-    aq, sq, iq, srt, _ = q.graph_np()
-    assert srt and np.array_equal(sr, sq) and np.array_equal(ir, iq)
-    assert np.array_equal(ar["ul"], aq["ul"]) and np.array_equal(canon_arcs(ar), canon_arcs(aq))
-    q.free(), p.free(), r.free()
+    for step, state in STEPS:
+        gold.expect(after(prod, step, state), lambda: after(ref, step, state))
+        getattr(r, step)()
+    r.free()
 
 
-def test_sub_edge_cases(ref, prod):
+def _sub(lib, a, *args):
+    pa = capi.c_malloc_copy(a)
+    s = lib.ma_hit_sub(*args[:3], len(a), pa, args[3])
+    out = capi.np_from_ptr(s, args[3], SUB_DT)
+    capi.c_free(s), capi.c_free(pa)
+    return out
+
+
+def test_sub_edge_cases(ref, prod, gold):
     """Hand-made groups: depth exactly min_dp, ties between equally long stretches (first wins), end
     touching a start at the same coordinate, self hits and low-identity hits skipped, reads that never
     head a group (hit.c:109-160)."""
@@ -111,11 +106,7 @@ def test_sub_edge_cases(ref, prod):
     a = np.array(rows, dtype=HIT_DT)
     a = a[np.argsort(a["qns"], kind="stable")]
     for clip in (0, 1000):
-        pa = capi.c_malloc_copy(a)
-        sr = ref.ma_hit_sub(3, 0.05, clip, len(a), pa, 16)
-        sp = prod.ma_hit_sub(3, 0.05, clip, len(a), pa, 16)
-        assert np.array_equal(capi.np_from_ptr(sr, 16, SUB_DT), capi.np_from_ptr(sp, 16, SUB_DT))
-        capi.c_free(sr), capi.c_free(sp), capi.c_free(pa)
+        gold.expect(_sub(prod, a, 3, 0.05, clip, 16), lambda: _sub(ref, a, 3, 0.05, clip, 16))
 
 
 def test_empty_inputs(prod):
@@ -127,7 +118,7 @@ def test_empty_inputs(prod):
 
 
 @pytest.mark.parametrize("span", [(30000, 20000), (9000, 11000), (200, 32000), (3, 40)], ids=["beyond32k", "reads10k", "edge32k", "tiny_coords"])
-def test_sub_group_sizes(span, ref, prod):
+def test_sub_group_sizes(span, ref, prod, gold):
     """Groups beyond the warp kernel (256 hits), beyond the CTA kernel (16384 hits) and tiny ones, in one array:
     the shared-memory paths and the device-wide-sort fallback of ma_hit_sub must agree with the reference.  `span` = (range of
     the interval starts, longest interval): below 32 768 the CTA kernel counts starts/ends per coordinate instead of sorting
@@ -145,11 +136,7 @@ def test_sub_group_sizes(span, ref, prod):
     a = np.array(rows, dtype=HIT_DT)
     a = a[np.argsort(a["qns"], kind="stable")]
     for dp, clip in ((3, 0), (3, 1000), (1, 0), (50, 300)):
-        pa = capi.c_malloc_copy(a)
-        sr = ref.ma_hit_sub(dp, 0.05, clip, len(a), pa, 200)
-        sp = prod.ma_hit_sub(dp, 0.05, clip, len(a), pa, 200)
-        assert np.array_equal(capi.np_from_ptr(sr, 200, SUB_DT), capi.np_from_ptr(sp, 200, SUB_DT)), (dp, clip)
-        capi.c_free(sr), capi.c_free(sp), capi.c_free(pa)
+        gold.expect(_sub(prod, a, dp, 0.05, clip, 200), lambda: _sub(ref, a, dp, 0.05, clip, 200))
 
 
 @pytest.mark.parametrize("name", ["tiny_exact", "chaos", "shuffled", "skew_small"])

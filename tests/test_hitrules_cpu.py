@@ -15,7 +15,7 @@ from miniasm_b200.capi import ARC_DT, DEL, HIT_DT, SUB_DT
 from miniasm_b200.pipeline import canon_arcs
 from oracle import loaders
 
-pytestmark = pytest.mark.skipif(not os.path.exists(loaders.REFERENCE_SO), reason="oracle/_ref not built (needs /root/reference)")
+pytestmark = pytest.mark.skipif(not os.path.exists(loaders.REFERENCE_SO), reason="oracle/_ref not built (needs the reference's sources)")
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SIM_SRC = os.path.join(ROOT, "tests", "hostsim", "hit_host.cpp")
