@@ -49,7 +49,6 @@ ma_hit_t *ma_hit_read(const char *fn, int min_span, int min_match, sdict_t *d, s
 	paf_rec_t r;
 	ma_hit_t *a = 0;
 	size_t n_a = 0, m_a = 0, tot = 0, tot_len = 0;
-	uint32_t max_qs = 0;
 	if (fp == 0) {
 		fprintf(stderr, "[E::%s] could not open PAF file %s\n", __func__, fn);
 		exit(1);
@@ -64,12 +63,10 @@ ma_hit_t *ma_hit_read(const char *fn, int min_span, int min_match, sdict_t *d, s
 		uint32_t qid = (uint32_t)sd_put(d, r.qn, r.ql), tid = (uint32_t)sd_put(d, r.tn, r.tl);
 		p->qns = (uint64_t)qid << 32 | r.qs, p->qe = r.qe, p->tn = tid;
 		p->ts = r.ts, p->te = r.te, p->rev = r.rev, p->ml = r.ml, p->bl = r.bl, p->del = 0;
-		if (r.qs > max_qs) max_qs = r.qs;
 		if (bi_dir && qid != tid) { // the same overlap seen from the target (hit.c:92-98)
 			ma_hit_t *m = &a[n_a++];
 			m->qns = (uint64_t)tid << 32 | r.ts, m->qe = r.te, m->tn = qid;
 			m->ts = r.qs, m->te = r.qe, m->rev = r.rev, m->ml = r.ml, m->bl = r.bl, m->del = 0;
-			if (r.ts > max_qs) max_qs = r.ts;
 		}
 	}
 	paf_close(fp);
@@ -80,10 +77,8 @@ ma_hit_t *ma_hit_read(const char *fn, int min_span, int min_match, sdict_t *d, s
 	if (n_a > 1) {
 		MabDev &dev = mab_default_dev();
 		DHits h;
-		uint32_t lb = 1;
-		while (lb < 32 && (max_qs >> lb)) ++lb;
 		hits_upload(dev, a, n_a, d->n_seq, h);
-		dh_sort(dev, h, lb);
+		dh_sort(dev, h);
 		hits_download(dev, h, a);
 		dh_free(dev, h);
 		dev.sync();

@@ -43,8 +43,11 @@ __device__ __forceinline__ void st_hit(DHit *p, const DHit &h)
 
 static inline uint32_t bits_for(uint64_t x) { uint32_t b = 0; while (x) ++b, x >>= 1; return b ? b : 1; }
 
+static void drop_bounds(MabDev &d, DHits &h) { d.free(h.grp); h.grp = nullptr; }
+
 void dh_reserve(MabDev &d, DHits &h, size_t m)
 {
+	drop_bounds(d, h);                  // the caller refills the hits
 	if (m <= h.m) return;
 	DHit *na = mab_alloc<DHit>(d, m), *nb = mab_alloc<DHit>(d, m);
 	if (h.n) MAB_CUDA(cudaMemcpyAsync(na, h.a, h.n * sizeof(DHit), cudaMemcpyDeviceToDevice, d.stream));
@@ -54,7 +57,7 @@ void dh_reserve(MabDev &d, DHits &h, size_t m)
 
 void dh_free(MabDev &d, DHits &h)
 {
-	d.free(h.a); d.free(h.a2);
+	d.free(h.a); d.free(h.a2); d.free(h.grp);
 	h = DHits();
 }
 
@@ -162,45 +165,206 @@ static size_t select_hits(MabDev &d, DHits &h, const uint8_t *flag)
 	size_t n = (size_t)d.get_scal(SC_NSEL);
 	DHit *t = h.a; h.a = h.a2; h.a2 = t;
 	h.n = n;
+	drop_bounds(d, h);
 	return n;
 }
 
-// ---------------------------------------------------------------------------------------------
-// ma_hit_sort: (key = qid << lb | qs, payload = position) radix sort, then a 32-byte gather
-// ---------------------------------------------------------------------------------------------
-__global__ void k_hit_keys(const DHit *a, size_t n, uint32_t lb, uint64_t *key, uint32_t *pos)
+// Bitonic network over 32*M keys held in registers, element e = 32*m + lane: exchanges at distance j < 32 are lane
+// shuffles, distances >= 32 pair two registers of the same lane -- no shared-memory traffic and none of the 2-way bank
+// conflicts the strided pair indexing has in the shared-memory version.
+template <int M, typename T>
+__device__ __forceinline__ void warp_bitonic_regs(T (&v)[M], const int lane)
 {
-	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-		uint64_t q = a[i].qns;
-		key[i] = lb >= 32 ? q : ((q >> 32) << lb | (uint32_t)q);
-		pos[i] = (uint32_t)i;
+	#pragma unroll
+	for (int k = 2; k <= 32 * M; k <<= 1) {
+		#pragma unroll
+		for (int j = k >> 1; j > 0; j >>= 1) {
+			if (j >= 32) {
+				#pragma unroll
+				for (int m = 0; m < M; ++m) {
+					const int pm = m ^ (j >> 5);
+					if (pm > m) {
+						const bool asc = ((32 * m) & k) == 0; // k >= 64 here: the lane bits do not reach it
+						const T x = v[m], y = v[pm];
+						const T lo = x < y ? x : y, hi = x < y ? y : x;
+						v[m] = asc ? lo : hi, v[pm] = asc ? hi : lo;
+					}
+				}
+			} else {
+				const bool low = (lane & j) == 0;
+				#pragma unroll
+				for (int m = 0; m < M; ++m) {
+					const T y = __shfl_xor_sync(0xffffffffu, v[m], j);
+					const bool asc = ((32 * m + lane) & k) == 0;
+					v[m] = (asc == low) == (v[m] < y) ? v[m] : y;
+				}
+			}
+		}
 	}
 }
-__global__ void k_hit_gather(const DHit *a, const uint32_t *pos, size_t n, DHit *out)
+
+// ---------------------------------------------------------------------------------------------
+// ma_hit_sort as a per-read bucket sort.  The number of reads is known and each read has ~100 hits, so the query-id part of
+// the key is a counting sort (per-read counts -> exclusive scan -> every hit's key scattered into its read's bucket with an
+// atomic cursor) and the query-start part a small sort per bucket.  A bucket holds key = qs << 32 | input position in the
+// nondeterministic order of the cursor; the keys are unique, so sorting them gives exactly the stable order by (qid, qs).
+// Three tiers by bucket size: a warp sorts up to BKW_HITS keys in registers, a CTA up to BKC_HITS with a block merge sort
+// (skewed sets: ~10 000 hits on each read of a hot locus), and larger buckets go to a segmented device sort of their keys only.
+// The sorted records land in h.a2 (then swapped with h.a); the bucket bounds become h.grp for ma_hit_sub.
+// ---------------------------------------------------------------------------------------------
+constexpr int BKW_WARPS = 8, BKW_HITS = 256;
+constexpr int BKC_THREADS = 512, BKC_ITEMS = 32, BKC_HITS = BKC_THREADS * BKC_ITEMS;
+typedef unsigned long long BKey;
+
+__global__ void k_bucket_count(const DHit *a, size_t n, uint32_t *cnt)
 {
 	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-		st_hit(out + i, ld_hit(a + pos[i]));
+		atomicAdd(&cnt[a[i].qns >> 32], 1u);
 }
 
-void dh_sort(MabDev &d, DHits &h, uint32_t max_len_bits)
+__global__ void k_bucket_fill(const DHit *a, size_t n, const uint32_t *__restrict__ first, uint32_t *cur, BKey *key)
 {
-	if (h.n < 2) return;
-	if (h.n >= (1ull << 32)) { fprintf(stderr, "[E::miniasm_b200] more than 2^32 hits on one GPU\n"); exit(73); }
-	uint32_t lb = max_len_bits > 32 ? 32 : max_len_bits;
-	int end_bit = (int)(lb + bits_for(h.n_seq ? h.n_seq - 1 : 0));
-	uint64_t *ka = mab_alloc<uint64_t>(d, h.n), *kb = mab_alloc<uint64_t>(d, h.n);
-	uint32_t *pa = mab_alloc<uint32_t>(d, h.n), *pb = mab_alloc<uint32_t>(d, h.n);
-	MAB_LAUNCH(d, k_hit_keys, mab_grid(h.n, 256), 256, 0, h.a, h.n, lb, ka, pa);
-	cub::DoubleBuffer<uint64_t> dk(ka, kb);
-	cub::DoubleBuffer<uint32_t> dp(pa, pb);
+	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+		const uint64_t qns = a[i].qns;
+		const uint32_t q = (uint32_t)(qns >> 32);
+		key[first[q] + atomicAdd(&cur[q], 1u)] = (BKey)(uint32_t)qns << 32 | i;
+	}
+}
+
+template <int M>
+__device__ __forceinline__ void bucket_sort_regs(const DHit *__restrict__ a, const BKey *__restrict__ key, uint32_t f, uint32_t cnt, DHit *__restrict__ out, int lane)
+{
+	BKey v[M];
+	#pragma unroll
+	for (int m = 0; m < M; ++m) v[m] = 32u * m + lane < cnt ? key[f + 32 * m + lane] : ~0ull;
+	warp_bitonic_regs<M>(v, lane);
+	#pragma unroll
+	for (int m = 0; m < M; ++m)
+		if (32u * m + lane < cnt) st_hit(out + f + 32 * m + lane, ld_hit(a + (uint32_t)v[m]));
+}
+
+__global__ void __launch_bounds__(BKW_WARPS * 32)
+k_bucket_warp(const DHit *__restrict__ a, const BKey *__restrict__ key, const uint32_t *__restrict__ first, uint32_t n_seq,
+              DHit *__restrict__ out, uint64_t *grp, uint32_t *big_list, unsigned long long *scal)
+{
+	const int lane = threadIdx.x & 31;
+	for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_seq; r += (gridDim.x * blockDim.x) >> 5) {
+		const uint32_t f = first[r], e = first[r + 1], cnt = e - f;
+		if (lane == 0) grp[r] = cnt ? (uint64_t)f << 32 | e : 0;
+		if (cnt == 0) continue;
+		if (cnt > BKW_HITS) { if (lane == 0) big_list[atomicAdd(scal + SC_BIG, 1ull)] = r; continue; }
+		if (cnt <= 32) bucket_sort_regs<1>(a, key, f, cnt, out, lane);
+		else if (cnt <= 64) bucket_sort_regs<2>(a, key, f, cnt, out, lane);
+		else if (cnt <= 128) bucket_sort_regs<4>(a, key, f, cnt, out, lane);
+		else bucket_sort_regs<8>(a, key, f, cnt, out, lane);
+	}
+}
+
+struct BKeyLess { __device__ __forceinline__ bool operator()(const BKey &x, const BKey &y) const { return x < y; } };
+typedef cub::BlockMergeSort<BKey, BKC_THREADS, BKC_ITEMS> BkcSort;
+
+__global__ void __launch_bounds__(BKC_THREADS, 1)
+k_bucket_cta(const DHit *__restrict__ a, const BKey *__restrict__ key, const uint32_t *__restrict__ first, const uint32_t *__restrict__ big_list,
+             uint32_t n_big, DHit *__restrict__ out, uint32_t *huge_list, unsigned long long *scal)
+{
+	extern __shared__ __align__(16) unsigned char bk_smem[];
+	typename BkcSort::TempStorage &ts = *reinterpret_cast<typename BkcSort::TempStorage*>(bk_smem);
+	const uint32_t tid = threadIdx.x;
+	for (uint32_t b = blockIdx.x; b < n_big; b += gridDim.x) {
+		const uint32_t r = big_list[b], f = first[r], cnt = first[r + 1] - f;
+		if (cnt > BKC_HITS) { if (tid == 0) huge_list[atomicAdd(scal + SC_AUX2, 1ull)] = r; continue; }
+		BKey v[BKC_ITEMS];
+		#pragma unroll
+		for (int k = 0; k < BKC_ITEMS; ++k) { const uint32_t j = k * BKC_THREADS + tid; v[k] = j < cnt ? key[f + j] : ~0ull; } // padding sorts last
+		BkcSort(ts).Sort(v, BKeyLess());
+		#pragma unroll
+		for (int k = 0; k < BKC_ITEMS; ++k) { // blocked: thread tid holds ranks tid * BKC_ITEMS + k
+			const uint32_t j = tid * BKC_ITEMS + k;
+			if (j < cnt) st_hit(out + f + j, ld_hit(a + (uint32_t)v[k]));
+		}
+		__syncthreads(); // the temp storage is reused by the next bucket
+	}
+}
+
+__global__ void k_bucket_segs(const uint32_t *list, uint32_t n, const uint32_t *first, int *beg, int *end)
+{
+	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+		beg[i] = (int)first[list[i]], end[i] = (int)first[list[i] + 1];
+}
+
+__global__ void k_bucket_gather(const DHit *__restrict__ a, const BKey *__restrict__ key, const uint32_t *__restrict__ first, const uint32_t *list, uint32_t n,
+                                DHit *__restrict__ out)
+{
+	for (uint32_t b = blockIdx.x; b < n; b += gridDim.x) {
+		const uint32_t f = first[list[b]], e = first[list[b] + 1];
+		for (uint32_t j = f + threadIdx.x; j < e; j += blockDim.x) st_hit(out + j, ld_hit(a + (uint32_t)key[j]));
+	}
+}
+
+void dh_bucket_first(MabDev &d, const uint32_t *cnt, uint32_t n_seq, uint32_t *first)
+{
 	size_t tb = 0;
-	cub::DeviceRadixSort::SortPairs(nullptr, tb, dk, dp, (int64_t)h.n, 0, end_bit, d.stream);
+	cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt, first, (int64_t)n_seq + 1, d.stream);
 	void *tmp = d.tmp(tb);
-	cub::DeviceRadixSort::SortPairs(tmp, tb, dk, dp, (int64_t)h.n, 0, end_bit, d.stream);
+	cub::DeviceScan::ExclusiveSum(tmp, tb, cnt, first, (int64_t)n_seq + 1, d.stream);
 	++d.n_lib;
-	MAB_LAUNCH(d, k_hit_gather, mab_grid(h.n, 256), 256, 0, h.a, dp.Current(), h.n, h.a2);
+}
+
+void dh_sort_buckets(MabDev &d, DHits &h, const uint32_t *first, const uint64_t *key64)
+{
+	drop_bounds(d, h);
+	const uint32_t n_seq = h.n_seq;
+	if (h.n == 0 || n_seq == 0) return;
+	if (h.n >= (1ull << 32)) { fprintf(stderr, "[E::miniasm_b200] more than 2^32 hits on one GPU\n"); exit(73); }
+	const BKey *key = reinterpret_cast<const BKey*>(key64);
+	h.grp = mab_alloc<uint64_t>(d, n_seq);
+	uint32_t *big = mab_alloc<uint32_t>(d, n_seq);
+	d.zero_scal(SC_BIG);
+	unsigned grid = (n_seq + BKW_WARPS - 1) / BKW_WARPS;
+	if (grid > MAB_SMS * 32u) grid = MAB_SMS * 32u;
+	MAB_LAUNCH(d, k_bucket_warp, grid, BKW_WARPS * 32, 0, h.a, key, first, n_seq, h.a2, h.grp, big, d.d_scal);
+	const uint32_t n_big = (uint32_t)d.get_scal(SC_BIG);
+	if (n_big) {
+		const size_t smem = sizeof(typename BkcSort::TempStorage);
+		MAB_CUDA(cudaFuncSetAttribute(k_bucket_cta, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); // per device: set on every use
+		uint32_t *huge = mab_alloc<uint32_t>(d, n_big);
+		d.zero_scal(SC_AUX2);
+		MAB_LAUNCH(d, k_bucket_cta, n_big < MAB_SMS ? n_big : MAB_SMS, BKC_THREADS, smem, h.a, key, first, big, n_big, h.a2, huge, d.d_scal);
+		const uint32_t n_huge = (uint32_t)d.get_scal(SC_AUX2);
+		if (n_huge) { // buckets beyond a CTA: a segmented sort of their keys (positions keep their bucket offsets), then the gather
+			if (h.n >= (1ull << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 hits on one GPU\n"); exit(73); }
+			BKey *sorted = mab_alloc<BKey>(d, h.n);
+			int *beg = mab_alloc<int>(d, n_huge), *end = mab_alloc<int>(d, n_huge);
+			MAB_LAUNCH(d, k_bucket_segs, mab_grid(n_huge, 128), 128, 0, huge, n_huge, first, beg, end);
+			size_t tb = 0;
+			cub::DeviceSegmentedSort::SortKeys(nullptr, tb, key, sorted, (int)h.n, (int)n_huge, beg, end, d.stream);
+			void *tmp = d.tmp(tb);
+			cub::DeviceSegmentedSort::SortKeys(tmp, tb, key, sorted, (int)h.n, (int)n_huge, beg, end, d.stream);
+			++d.n_lib;
+			MAB_LAUNCH(d, k_bucket_gather, n_huge < MAB_SMS * 4 ? n_huge : MAB_SMS * 4, 256, 0, h.a, sorted, first, huge, n_huge, h.a2);
+			d.free(sorted); d.free(beg); d.free(end);
+		}
+		d.free(huge);
+	}
+	d.free(big);
 	DHit *t = h.a; h.a = h.a2; h.a2 = t;
-	d.free(ka); d.free(kb); d.free(pa); d.free(pb);
+}
+
+void dh_sort(MabDev &d, DHits &h)
+{
+	drop_bounds(d, h);
+	const uint32_t n_seq = h.n_seq;
+	if (h.n == 0 || n_seq == 0) return;
+	if (h.n >= (1ull << 32)) { fprintf(stderr, "[E::miniasm_b200] more than 2^32 hits on one GPU\n"); exit(73); }
+	uint32_t *cnt = mab_alloc<uint32_t>(d, (size_t)n_seq + 1), *first = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);
+	uint64_t *key = mab_alloc<uint64_t>(d, h.n);
+	MAB_CUDA(cudaMemsetAsync(cnt, 0, ((size_t)n_seq + 1) * 4, d.stream));
+	MAB_LAUNCH(d, k_bucket_count, mab_grid(h.n, 256), 256, 0, h.a, h.n, cnt);
+	dh_bucket_first(d, cnt, n_seq, first);
+	MAB_CUDA(cudaMemsetAsync(cnt, 0, (size_t)n_seq * 4, d.stream));   // the counts become the buckets' fill cursors
+	MAB_LAUNCH(d, k_bucket_fill, mab_grid(h.n, 256), 256, 0, h.a, h.n, first, cnt, reinterpret_cast<BKey*>(key));
+	dh_sort_buckets(d, h, first, key);
+	d.free(cnt); d.free(first); d.free(key);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -362,40 +526,6 @@ __device__ __forceinline__ bool sub_hit_keys(const DHit &h, uint32_t qid, float 
 	if (!(qe > qs)) return false;
 	*ks = qs << 1, *ke = qe << 1 | 1;
 	return true;
-}
-
-// Bitonic network over 32*M keys held in registers, element e = 32*m + lane: exchanges at distance j < 32 are lane
-// shuffles, distances >= 32 pair two registers of the same lane -- no shared-memory traffic and none of the 2-way bank
-// conflicts the strided pair indexing has in the shared-memory version.
-template <int M>
-__device__ __forceinline__ void warp_bitonic_regs(uint32_t (&v)[M], const int lane)
-{
-	#pragma unroll
-	for (int k = 2; k <= 32 * M; k <<= 1) {
-		#pragma unroll
-		for (int j = k >> 1; j > 0; j >>= 1) {
-			if (j >= 32) {
-				#pragma unroll
-				for (int m = 0; m < M; ++m) {
-					const int pm = m ^ (j >> 5);
-					if (pm > m) {
-						const bool asc = ((32 * m) & k) == 0; // k >= 64 here: the lane bits do not reach it
-						const uint32_t x = v[m], y = v[pm];
-						const uint32_t lo = min(x, y), hi = max(x, y);
-						v[m] = asc ? lo : hi, v[pm] = asc ? hi : lo;
-					}
-				}
-			} else {
-				const bool low = (lane & j) == 0;
-				#pragma unroll
-				for (int m = 0; m < M; ++m) {
-					const uint32_t y = __shfl_xor_sync(0xffffffffu, v[m], j);
-					const bool asc = ((32 * m + lane) & k) == 0;
-					v[m] = asc == low ? min(v[m], y) : max(v[m], y);
-				}
-			}
-		}
-	}
 }
 
 template <int M>
@@ -628,11 +758,14 @@ uint64_t dh_sub(MabDev &d, const DHits &h, int min_dp, float min_iden, int end_c
 	if (n_seq) MAB_CUDA(cudaMemsetAsync(sub_out, 0, (size_t)n_seq * sizeof(DSub), d.stream));
 	if (h.n == 0 || n_seq == 0) return 0;
 	if (h.n >= (1ull << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 hits on one GPU\n"); exit(73); }
-	uint64_t *grp = mab_alloc<uint64_t>(d, n_seq);
+	uint64_t *grp = h.grp;              // the bounds the sort left, while no pass has moved the hits since
+	if (!grp) {
+		grp = mab_alloc<uint64_t>(d, n_seq);
+		MAB_CUDA(cudaMemsetAsync(grp, 0, (size_t)n_seq * 8, d.stream));
+		MAB_LAUNCH(d, k_group_bounds, mab_grid(h.n, 256), 256, 0, h.a, h.n, (uint32_t*)grp);
+	}
 	uint32_t *big = mab_alloc<uint32_t>(d, n_seq);
-	MAB_CUDA(cudaMemsetAsync(grp, 0, (size_t)n_seq * 8, d.stream));
 	MAB_CUDA(cudaMemsetAsync(d.d_scal, 0, 8 * sizeof(unsigned long long), d.stream));
-	MAB_LAUNCH(d, k_group_bounds, mab_grid(h.n, 256), 256, 0, h.a, h.n, (uint32_t*)grp);
 	unsigned grid = (n_seq + SUBW_WARPS - 1) / SUBW_WARPS;
 	if (grid > MAB_SMS * 32u) grid = MAB_SMS * 32u;
 	static const int smem_sort = getenv("MAB_SUB_SMEM_SORT") && atoi(getenv("MAB_SUB_SMEM_SORT")) != 0; // 1: the shared-memory network
@@ -656,7 +789,8 @@ uint64_t dh_sub(MabDev &d, const DHits &h, int min_dp, float min_iden, int end_c
 		d.free(huge);
 	}
 	uint64_t n_remained = d.get_scal(SC_COUNT);
-	d.free(grp); d.free(big);
+	if (grp != h.grp) d.free(grp);
+	d.free(big);
 	{ unsigned long long v[1] = { n_remained }; sum_ranks(v, 1); n_remained = v[0]; }
 	if (ma_verbose_dev >= 3)
 		fprintf(stderr, "[M::%s::%s] %ld query sequences remain after sub\n", "ma_hit_sub", sys_timestamp(), (long)n_remained);
@@ -972,6 +1106,7 @@ size_t dh_contained(MabDev &d, DHits &h, DSub *sub, const uint8_t *seq_del, cons
 		d.free(used); d.free(keep); d.free(excl); d.free(sub2);
 	}
 	h.n_seq = n_new;
+	drop_bounds(d, h);                  // reads renumbered
 	unsigned long long gv[2] = { (unsigned long long)n_cut, (unsigned long long)h.n };
 	sum_ranks(gv, 2);
 	if (cut_reg && ma_verbose_dev >= 3) fprintf(stderr, "[M::%s::%s] %ld hits remain after cut\n", "ma_hit_cut", sys_timestamp(), (long)gv[0]);

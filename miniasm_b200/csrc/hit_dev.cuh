@@ -14,6 +14,9 @@ struct DHits {
 	DHit *a = nullptr, *a2 = nullptr;   // hit array + ping-pong buffer for compaction
 	size_t n = 0, m = 0;
 	uint32_t n_seq = 0;
+	// per-read bounds of the sorted hits, first << 32 | end (0 = the read heads no hits), n_seq entries; left by the sort and
+	// dropped by every pass that moves, drops or renumbers hits (null = unknown: ma_hit_sub derives them from the hits)
+	uint64_t *grp = nullptr;
 };
 
 struct HitArcParams { int max_hang; float int_frac; int min_ovlp; };
@@ -21,8 +24,14 @@ struct HitArcParams { int max_hang; float int_frac; int min_ovlp; };
 void dh_reserve(MabDev &d, DHits &h, size_t m);
 void dh_free(MabDev &d, DHits &h);
 
-// ma_hit_sort (hit.c:19-22): sort by the 64-bit qns (query id, then query start); stable.
-void dh_sort(MabDev &d, DHits &h, uint32_t max_len_bits);
+// ma_hit_sort (hit.c:19-22): sort by the 64-bit qns (query id, then query start); stable.  A per-read bucket sort: counts per
+// query read, every hit's key (qs << 32 | input position) in its read's bucket, then each bucket sorted and its records gathered.
+// Sets h.grp.
+void dh_sort(MabDev &d, DHits &h);
+// The same for a caller that built the buckets itself: first = exclusive scan of the per-read counts (n_seq + 1 entries, from
+// dh_bucket_first), key[first[q] ..< first[q + 1]] = the keys of read q's hits in any order.
+void dh_bucket_first(MabDev &d, const uint32_t *cnt, uint32_t n_seq, uint32_t *first);
+void dh_sort_buckets(MabDev &d, DHits &h, const uint32_t *first, const uint64_t *key);
 
 // ma_hit_sub (hit.c:109-160).  sub_out: n_seq entries, fully written (zeros for reads heading no group).
 // Returns the number of reads that keep an interval ("query sequences remain after sub").

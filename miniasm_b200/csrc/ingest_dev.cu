@@ -447,34 +447,38 @@ __global__ void k_dict_rank(const unsigned long long *first_sorted, const uint64
 }
 
 // --------------------------------------------------------------------------------------------- hits
-__global__ void k_hit_count(const PRec *ln, uint64_t n_lines, int bi_dir, uint32_t *cnt)
+// hits per line, and per query read (the bucket sizes of the sort, dh_sort_buckets)
+__global__ void k_hit_count(const PRec *ln, uint64_t n_lines, int bi_dir, NameTab t, uint32_t *cnt, uint32_t *read_cnt)
 {
 	for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n_lines; i += (uint64_t)gridDim.x * blockDim.x) {
 		const uint2 sl = *reinterpret_cast<const uint2*>(&ln[i].slot_q);
-		cnt[i] = sl.x != NOSLOT ? (bi_dir && sl.x != sl.y ? 2 : 1) : 0;
+		const uint32_t c = sl.x != NOSLOT ? (bi_dir && sl.x != sl.y ? 2 : 1) : 0;
+		cnt[i] = c;
+		if (c) atomicAdd(&read_cnt[t.id[sl.x]], 1u);
+		if (c == 2) atomicAdd(&read_cnt[t.id[sl.y]], 1u);
 	}
 }
 
-__global__ void k_hit_emit(const PRec *ln, uint64_t n_lines, const uint32_t *cnt, const uint64_t *off, NameTab t, DHit *out, unsigned *max_qs)
+// hits at off[i] (file order), and every hit's sort key (qs << 32 | position) into its query read's bucket
+__global__ void k_hit_emit(const PRec *ln, uint64_t n_lines, const uint32_t *cnt, const uint64_t *off, NameTab t, DHit *out,
+                           const uint32_t *__restrict__ first, uint32_t *cur, unsigned long long *key)
 {
-	unsigned mx = 0;
 	for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n_lines; i += (uint64_t)gridDim.x * blockDim.x) {
 		const uint32_t c = cnt[i];
 		if (c == 0) continue;
 		const PRec r = ln[i];
 		const uint32_t qid = t.id[r.slot_q], tid = t.id[r.slot_t], bl = line_bl(ln, i, 0);
-		uint4 *o = reinterpret_cast<uint4*>(out + off[i]);
+		const uint64_t p = off[i];
+		uint4 *o = reinterpret_cast<uint4*>(out + p);
 		o[0] = make_uint4(r.qs, qid, r.qe, tid);
 		o[1] = make_uint4(r.ts, r.te, r.ml_rev, bl);
-		mx = r.qs > mx ? r.qs : mx;
+		key[first[qid] + atomicAdd(&cur[qid], 1u)] = (unsigned long long)r.qs << 32 | p;
 		if (c == 2) { // the same overlap seen from the target (hit.c:92-98)
 			o[2] = make_uint4(r.ts, tid, r.te, qid);
 			o[3] = make_uint4(r.qs, r.qe, r.ml_rev, bl);
-			mx = r.ts > mx ? r.ts : mx;
+			key[first[tid] + atomicAdd(&cur[tid], 1u)] = (unsigned long long)r.ts << 32 | (p + 1);
 		}
 	}
-	mx = __reduce_max_sync(0xffffffffu, mx);
-	if ((threadIdx.x & 31) == 0 && mx) atomicMax(max_qs, mx);
 }
 
 // start[i] = byte offset of line i (a line starts at byte 0 and after every '\n' that is not the last byte); len > 0
@@ -705,10 +709,15 @@ static void ingest_finish(MabDev &d, const char *d_text, size_t len, uint64_t *s
 	d.free(slots);
 
 	d.trace("ingest:rank_ids");
-	// (5) hits at scanned offsets (file order, mirrored hit right after its original)
+	// (5) hits at scanned offsets (file order, mirrored hit right after its original); the counts per query read and the keys in
+	// their buckets are taken on the way, so the sort starts from the buckets
 	cnt = mab_alloc<uint32_t>(d, n_lines);
 	off = mab_alloc<uint64_t>(d, n_lines + 1);
-	MAB_LAUNCH(d, k_hit_count, mab_grid(n_lines, 256), 256, 0, ln, n_lines, bi_dir, cnt);
+	uint32_t *read_cnt = mab_alloc<uint32_t>(d, (size_t)n_seq + 1), *first = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);
+	MAB_CUDA(cudaMemsetAsync(read_cnt, 0, ((size_t)n_seq + 1) * 4, d.stream));
+	MAB_LAUNCH(d, k_hit_count, mab_grid(n_lines, 256), 256, 0, ln, n_lines, bi_dir, tab, cnt, read_cnt);
+	dh_bucket_first(d, read_cnt, n_seq, first);
+	MAB_CUDA(cudaMemsetAsync(read_cnt, 0, (size_t)n_seq * 4, d.stream)); // the counts become the buckets' fill cursors
 	{
 		size_t tb = 0;
 		cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt, off, (int64_t)n_lines, d.stream);
@@ -722,18 +731,19 @@ static void ingest_finish(MabDev &d, const char *d_text, size_t len, uint64_t *s
 	MAB_CUDA(cudaMemcpyAsync(&last_cnt, cnt + n_lines - 1, 4, cudaMemcpyDeviceToHost, d.stream));
 	d.sync();
 	const uint64_t n_hits = last_off + last_cnt;
+	if (n_hits >= (1ull << 32)) { fprintf(stderr, "[E::miniasm_b200] more than 2^32 hits on one GPU\n"); exit(73); }
 	dh_reserve(d, h, n_hits ? n_hits : 1);
 	h.n = n_hits, h.n_seq = n_seq;
-	d.zero_scal(SC_AUX, 1);
-	if (n_hits) MAB_LAUNCH(d, k_hit_emit, mab_grid(n_lines, 256), 256, 0, ln, n_lines, cnt, off, tab, h.a, (unsigned*)(d.d_scal + SC_AUX));
-	uint32_t max_qs = (uint32_t)(d.get_scal(SC_AUX) & 0xffffffffu);
-	st.n_hits = n_hits, st.n_seq = n_seq, st.max_qs_bits = bits_for(max_qs);
+	uint64_t *key = mab_alloc<uint64_t>(d, n_hits);
+	if (n_hits) MAB_LAUNCH(d, k_hit_emit, mab_grid(n_lines, 256), 256, 0, ln, n_lines, cnt, off, tab, h.a, first, read_cnt, (unsigned long long*)key);
+	st.n_hits = n_hits, st.n_seq = n_seq;
 	d.free(cnt); d.free(off); d.free(ln); d.free(start);
 	d.free(tab.key); d.free(tab.first); d.free(tab.id);
 
 	d.trace("ingest:emit_hits");
-	// (6) ma_hit_sort
-	dh_sort(d, h, st.max_qs_bits);
+	// (6) ma_hit_sort: order every bucket
+	dh_sort_buckets(d, h, first, key);
+	d.free(read_cnt); d.free(first); d.free(key);
 	d.trace("ingest:sort_hits");
 }
 
@@ -871,9 +881,8 @@ __global__ void k_line_gids(const PRec *ln, uint64_t n_lines, NameTab lt, int bi
 }
 
 __global__ void k_hit_emit_gid(const PRec *ln, uint64_t n_lines, const uint32_t *cnt, const uint64_t *off, NameTab lt, uint32_t carry_bl, uint32_t world,
-                               DHit *out, uint32_t *dest, unsigned *max_qs)
+                               DHit *out, uint32_t *dest)
 {
-	unsigned mx = 0;
 	for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n_lines; i += (uint64_t)gridDim.x * blockDim.x) {
 		const uint32_t c = cnt[i];
 		if (c == 0) continue;
@@ -883,16 +892,12 @@ __global__ void k_hit_emit_gid(const PRec *ln, uint64_t n_lines, const uint32_t 
 		o[0] = make_uint4(r.qs, qid, r.qe, tid);
 		o[1] = make_uint4(r.ts, r.te, r.ml_rev, bl);
 		dest[off[i]] = qid % world;
-		mx = r.qs > mx ? r.qs : mx;
 		if (c == 2) {
 			o[2] = make_uint4(r.ts, tid, r.te, qid);
 			o[3] = make_uint4(r.qs, r.qe, r.ml_rev, bl);
 			dest[off[i] + 1] = tid % world;
-			mx = r.ts > mx ? r.ts : mx;
 		}
 	}
-	mx = __reduce_max_sync(0xffffffffu, mx);
-	if ((threadIdx.x & 31) == 0 && mx) atomicMax(max_qs, mx);
 }
 
 // ---- emit + exchange fused: every hit is written straight into the receive buffer of the rank that owns its query read ------
@@ -939,13 +944,12 @@ __global__ void __launch_bounds__(PUSH_LINES) k_push_count(const PRec *ln, uint6
 // staging area goes out with consecutive threads writing consecutive 16-byte halves: every destination receives one contiguous
 // run per block (2 KB at 8 ranks) instead of isolated 32-byte stores -- isolated stores ran the NVLink at ~290 GB/s (11 ms at N=4).
 __global__ void __launch_bounds__(PUSH_LINES) k_push_emit(const PRec *ln, uint64_t n_lines, NameTab lt, int bi_dir, uint32_t carry_bl, uint32_t world, uint64_t n_blk,
-                                                          const uint64_t *__restrict__ blk_off, const long long *__restrict__ pos_base, DHit *const *__restrict__ dst, unsigned *max_qs)
+                                                          const uint64_t *__restrict__ blk_off, const long long *__restrict__ pos_base, DHit *const *__restrict__ dst)
 {
 	__shared__ uint32_t s_wc[PUSH_LINES / 32][32];
 	__shared__ uint32_t s_seg[33];                                  // exclusive prefix of the block's per-destination totals
 	__shared__ __align__(16) uint4 s_hit[2 * 2 * PUSH_LINES];        // up to two hits per line, two 16-byte halves per hit
 	const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, lt_mask = (1u << lane) - 1u;
-	unsigned mx = 0;
 	for (uint64_t b = blockIdx.x; b < n_blk; b += gridDim.x) {
 		const uint64_t i = b * PUSH_LINES + threadIdx.x;
 		const PushLine p = push_line(ln, i, n_lines, lt, bi_dir, world);
@@ -976,12 +980,10 @@ __global__ void __launch_bounds__(PUSH_LINES) k_push_emit(const PRec *ln, uint64
 			const uint32_t k0 = s_seg[p.d0] + w0 + r0;
 			s_hit[2 * k0] = make_uint4(r.qs, p.qid, r.qe, p.tid);
 			s_hit[2 * k0 + 1] = make_uint4(r.ts, r.te, r.ml_rev, bl);
-			mx = r.qs > mx ? r.qs : mx;
 			if (p.has1) { // the same overlap seen from the target (hit.c:92-98)
 				const uint32_t k1 = s_seg[p.d1] + w1 + r1;
 				s_hit[2 * k1] = make_uint4(r.ts, p.tid, r.te, p.qid);
 				s_hit[2 * k1 + 1] = make_uint4(r.qs, r.qe, r.ml_rev, bl);
-				mx = r.ts > mx ? r.ts : mx;
 			}
 		}
 		__syncthreads();
@@ -996,8 +998,6 @@ __global__ void __launch_bounds__(PUSH_LINES) k_push_emit(const PRec *ln, uint64
 		__syncthreads();
 	}
 	__threadfence_system();                            // the stores to peer memory are out before the grid reports completion
-	mx = __reduce_max_sync(0xffffffffu, mx);
-	if (lane == 0 && mx) atomicMax(max_qs, mx);
 }
 
 __global__ void k_gather_hits(const DHit *a, const uint32_t *pos, uint64_t n, DHit *out)
@@ -1204,7 +1204,6 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 	// (6) local hits with global ids go to the rank that owns their query read
 	if (G > 32) { fprintf(stderr, "[E::miniasm_b200] more than 32 ranks\n"); exit(79); }
 	if (n_ent) MAB_LAUNCH(d, k_local_gid, mab_grid(n_ent, 256), 256, 0, slots, n_ent, slot_of + my_ent_off, gt, tab);
-	uint32_t max_qs = 0;
 	uint64_t n_recv = 0;
 	std::vector<uint64_t> send_cnt(G, 0), recv_cnt(G, 0), mat((size_t)G * G, 0);
 	auto counts_matrix = [&]() { // every rank learns how much it receives from whom
@@ -1257,13 +1256,8 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 		DHit **d_dst = (DHit**)d.alloc(sizeof(void*) * (size_t)G);
 		MAB_CUDA(cudaMemcpyAsync(d_pos, pos_base.data(), sizeof(long long) * (size_t)G, cudaMemcpyHostToDevice, d.stream));
 		MAB_CUDA(cudaMemcpyAsync(d_dst, peer.data(), sizeof(void*) * (size_t)G, cudaMemcpyHostToDevice, d.stream));
-		d.zero_scal(SC_AUX, 1);
-		if (n_blk) MAB_LAUNCH(d, k_push_emit, mab_grid(n_blk, 1, MAB_SMS * 8u), PUSH_LINES, 0, ln, n_lines, tab, bi_dir, carry, (uint32_t)G, n_blk, blk_off, d_pos, d_dst, (unsigned*)(d.d_scal + SC_AUX));
-		max_qs = (uint32_t)(d.get_scal(SC_AUX) & 0xffffffffu);
-		{ // nobody sorts before everybody has finished writing: a one-word all-reduce, stream-ordered after the emit kernel on every rank
-			std::vector<uint64_t> mq = sc_allgather_u64(d, sc, max_qs);
-			for (int r = 0; r < G; ++r) if (mq[r] > max_qs) max_qs = (uint32_t)mq[r];
-		}
+		if (n_blk) MAB_LAUNCH(d, k_push_emit, mab_grid(n_blk, 1, MAB_SMS * 8u), PUSH_LINES, 0, ln, n_lines, tab, bi_dir, carry, (uint32_t)G, n_blk, blk_off, d_pos, d_dst);
+		sc_allgather_u64(d, sc, 0); // nobody sorts before everybody has finished writing: a one-word all-gather, stream-ordered after the emit kernel on every rank
 		d.free(d_pos); d.free((void*)d_dst);
 		d.trace("shard-ingest:emit + push over NVLink");
 	}
@@ -1282,9 +1276,8 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 	}
 	DHit *loc = mab_alloc<DHit>(d, n_loc), *snd = mab_alloc<DHit>(d, n_loc);
 	uint32_t *dest = mab_alloc<uint32_t>(d, n_loc), *dest2 = mab_alloc<uint32_t>(d, n_loc), *ia = mab_alloc<uint32_t>(d, n_loc), *ib = mab_alloc<uint32_t>(d, n_loc);
-	d.zero_scal(SC_AUX, 1);
 	if (n_loc) {
-		MAB_LAUNCH(d, k_hit_emit_gid, mab_grid(n_lines, 256), 256, 0, ln, n_lines, cnt, off, tab, carry, (uint32_t)G, loc, dest, (unsigned*)(d.d_scal + SC_AUX));
+		MAB_LAUNCH(d, k_hit_emit_gid, mab_grid(n_lines, 256), 256, 0, ln, n_lines, cnt, off, tab, carry, (uint32_t)G, loc, dest);
 		MAB_LAUNCH(d, k_iota32, mab_grid(n_loc, 256), 256, 0, ia, n_loc);
 		cub::DoubleBuffer<uint32_t> dk(dest, dest2), dv(ia, ib);
 		size_t tb = 0;
@@ -1296,16 +1289,11 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 		MAB_LAUNCH(d, k_gather_hits, mab_grid(n_loc, 256), 256, 0, loc, dv.Current(), n_loc, snd);
 	}
 	d.trace("shard-ingest:emit+bucket hits");
-	max_qs = (uint32_t)(d.get_scal(SC_AUX) & 0xffffffffu);
 	{
 		std::vector<uint64_t> sb(G), rb(G);
 		for (int r = 0; r < G; ++r) sb[r] = send_cnt[r] * sizeof(DHit), rb[r] = recv_cnt[r] * sizeof(DHit);
 		if (sc.active()) sc_alltoall_v(d, sc, snd, sb, h.a, rb);
 		else if (n_loc) MAB_CUDA(cudaMemcpyAsync(h.a, snd, n_loc * sizeof(DHit), cudaMemcpyDeviceToDevice, d.stream));
-	}
-	{ // sort key width must cover the largest query start of any rank
-		std::vector<uint64_t> mq = sc_allgather_u64(d, sc, max_qs);
-		for (int r = 0; r < G; ++r) if (mq[r] > max_qs) max_qs = (uint32_t)mq[r];
 	}
 	d.sync();
 	d.free(loc); d.free(snd); d.free(dest); d.free(dest2); d.free(ia); d.free(ib); d.free(cnt); d.free(off);
@@ -1320,7 +1308,7 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 	std::vector<uint64_t> hits_all = sc_allgather_u64(d, sc, n_recv), parsed_all = sc_allgather_u64(d, sc, st.n_parsed);
 	st.n_hits = st.n_parsed = 0;
 	for (int r = 0; r < G; ++r) st.n_hits += hits_all[r], st.n_parsed += parsed_all[r];
-	st.n_seq = n_seq, st.max_qs_bits = bits_for(max_qs);
-	dh_sort(d, h, st.max_qs_bits);
+	st.n_seq = n_seq;
+	dh_sort(d, h);
 	d.trace("shard-ingest:sort");
 }

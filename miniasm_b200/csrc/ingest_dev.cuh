@@ -13,7 +13,7 @@ struct DNames {
 	uint32_t *slen = nullptr;    // sequence length recorded at first appearance
 };
 
-struct IngestStats { uint64_t n_lines, n_parsed, n_hits, n_seq, tot_len, n_dropped; uint32_t max_qs_bits; int hash_retries; };
+struct IngestStats { uint64_t n_lines, n_parsed, n_hits, n_seq, tot_len, n_dropped; int hash_retries; };
 struct NoContParams { int max_hang; float int_frac; }; // -R (ma_hit_no_cont, hit.c:38-68)
 
 // d_text: the PAF bytes in device memory.  On return `h` holds the sorted hits (ma_hit_sort order, stable) and
