@@ -327,6 +327,30 @@ int mab_select(mab_ctx_t *c, const ma_opt_t *opt, int no_first, int no_second, i
 	DHits &h = c->hits;
 	PhaseTimer pt(d, &c->stats.ms_select, "mab_select");
 	ctx_drop_graphs(c);
+	auto step3_banner = [] { if (!mab_mute && ma_verbose >= 1) fprintf(stderr, "[M::main] ===> Step 3: 2-pass (fine) read selection <===\n"); };
+	auto renumber = [c, &d](const int32_t *map, uint32_t n_old) {
+		uint32_t *orig_new = mab_alloc<uint32_t>(d, c->hits.n_seq);
+		if (n_old) MAB_LAUNCH(d, k_orig_from_map, mab_grid(n_old, 256), 256, 0, n_old, map, c->orig_id, orig_new);
+		d.free(c->orig_id);
+		c->orig_id = orig_new;
+		c->n_seq = c->hits.n_seq;
+	};
+	if (!no_first && !no_second && stage >= 5) { // the whole selection: per-read passes over the hit buckets
+		if (!mab_mute && ma_verbose >= 1) fprintf(stderr, "[M::main] ===> Step 2: 1-pass (crude) read selection <===\n");
+		d.free(c->sub);
+		c->sub = mab_alloc<DSub>(d, c->n_seq);
+		d.trace("select:begin");
+		const uint32_t n_old = c->n_seq;
+		int32_t *map = mab_alloc<int32_t>(d, n_old);
+		const SelectParams sp = { opt->min_dp, opt->min_iden, opt->min_span, (int)(opt->max_hang * 1.5), (int)(opt->min_ovlp * .5),
+		                          { opt->max_hang, opt->int_frac, opt->min_ovlp } };
+		dh_select(d, h, c->sub, sp, map, &c->cov, step3_banner);
+		renumber(map, n_old);
+		d.free(map);
+		c->stats.n_hits_final = h.n, c->stats.n_seq_final = c->n_seq;
+		d.sync();
+		return 0;
+	}
 	if (!no_first) {
 		if (!mab_mute && ma_verbose >= 1) fprintf(stderr, "[M::main] ===> Step 2: 1-pass (crude) read selection <===\n");
 		if (stage >= 2) {
@@ -341,43 +365,22 @@ int mab_select(mab_ctx_t *c, const ma_opt_t *opt, int no_first, int no_second, i
 		}
 	}
 	if (!no_second) {
-		if (!mab_mute && ma_verbose >= 1) fprintf(stderr, "[M::main] ===> Step 3: 2-pass (fine) read selection <===\n");
+		step3_banner();
 		if (stage >= 4) {
 			DSub *sub2 = mab_alloc<DSub>(d, c->n_seq);
 			d.trace("select:flt");
 			dh_sub(d, h, opt->min_dp, opt->min_iden, opt->min_span / 2, sub2);
 			d.trace("select:sub2");
-			DSub *cut2 = nullptr; // round-2 table kept aside when its ma_hit_cut is fused into the containment pass
-			if (stage >= 5) {
-				cut2 = mab_alloc<DSub>(d, c->n_seq);
-				if (c->n_seq) MAB_CUDA(cudaMemcpyAsync(cut2, sub2, (size_t)c->n_seq * sizeof(DSub), cudaMemcpyDeviceToDevice, d.stream));
-			} else dh_cut(d, h, sub2, opt->min_span);
+			dh_cut(d, h, sub2, opt->min_span);
 			if (!no_first && c->sub) { dh_sub_merge(d, c->n_seq, c->sub, sub2); d.free(sub2); }
 			else { d.free(c->sub); c->sub = sub2; }
-			if (cut2) {
-				const uint32_t n_old = c->n_seq;
-				int32_t *map = mab_alloc<int32_t>(d, n_old);
-				HitArcParams p = { opt->max_hang, opt->int_frac, opt->min_ovlp };
-				dh_contained(d, h, c->sub, nullptr, p, map, cut2, opt->min_span);
-				uint32_t *orig_new = mab_alloc<uint32_t>(d, h.n_seq);
-				if (n_old) MAB_LAUNCH(d, k_orig_from_map, mab_grid(n_old, 256), 256, 0, n_old, map, c->orig_id, orig_new);
-				d.free(c->orig_id);
-				c->orig_id = orig_new;
-				c->n_seq = h.n_seq;
-				d.free(map); d.free(cut2);
-				d.trace("select:cut2+contained");
-			}
-		} else
+		}
 		if (stage >= 5 && c->sub) {
 			const uint32_t n_old = c->n_seq;
 			int32_t *map = mab_alloc<int32_t>(d, n_old);
 			HitArcParams p = { opt->max_hang, opt->int_frac, opt->min_ovlp };
 			dh_contained(d, h, c->sub, nullptr, p, map);
-			uint32_t *orig_new = mab_alloc<uint32_t>(d, h.n_seq);
-			if (n_old) MAB_LAUNCH(d, k_orig_from_map, mab_grid(n_old, 256), 256, 0, n_old, map, c->orig_id, orig_new);
-			d.free(c->orig_id);
-			c->orig_id = orig_new;
-			c->n_seq = h.n_seq;
+			renumber(map, n_old);
 			d.free(map);
 			d.trace("select:contained");
 		}

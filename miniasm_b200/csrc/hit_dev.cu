@@ -385,13 +385,15 @@ __global__ void k_group_bounds(const DHit *a, size_t n, uint32_t *g32)
 	}
 }
 
-__global__ void k_sub_keys(const DHit *a, size_t n, float min_iden, uint32_t clip, uint64_t *key)
+// Slots at or past their read's bound (grp) are dead: dh_select leaves them behind the live hits of each bucket, still under
+// the read's id, so they only turn into invalid keys.
+__global__ void k_sub_keys(const DHit *a, size_t n, const uint64_t *__restrict__ grp, float min_iden, uint32_t clip, uint64_t *key)
 {
 	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
 		DHit h = ld_hit(a + i);
 		uint32_t qid = (uint32_t)(h.qns >> 32);
 		int ml = (int)(h.ml_rev & 0x7fffffffu), bl = (int)(h.bl_del & 0x7fffffffu);
-		bool skip = h.tn == qid || (float)ml < __fmul_rn((float)bl, min_iden);
+		bool skip = i >= (uint32_t)grp[qid] || h.tn == qid || (float)ml < __fmul_rn((float)bl, min_iden);
 		uint32_t qs = (uint32_t)h.qns + clip, qe = h.qe - clip;
 		uint64_t base = (uint64_t)qid << 33;
 		if (!skip && qe > qs) {
@@ -752,6 +754,28 @@ __global__ void k_sub_copy_listed(const uint32_t *list, uint32_t n, const DSub *
 
 static uint64_t dh_sub_global(MabDev &d, const DHits &h, int min_dp, float min_iden, int end_clip, DSub *sub_out, const uint64_t *grp);
 
+// ma_hit_sub of the reads the warp tier listed (more than SUBW_HITS hits): a CTA each up to SUBC_HITS hits, the device-wide key
+// sort beyond.  Adds the reads that keep an interval to d_scal[SC_COUNT]; d_scal[SC_AUX2] must be zero on entry.
+static void sub_big_reads(MabDev &d, const DHits &h, const uint64_t *grp, const uint32_t *big, uint32_t n_big, int min_dp, float min_iden,
+                          int end_clip, DSub *sub_out)
+{
+	const size_t smem = (size_t)SUBC_HITS * 2 * 4;
+	MAB_CUDA(cudaFuncSetAttribute(k_sub_cta, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); // per device: set on every use
+	uint32_t *huge = mab_alloc<uint32_t>(d, n_big);
+	MAB_LAUNCH(d, k_sub_cta, n_big < MAB_SMS * 2 ? n_big : MAB_SMS * 2, 512, smem, h.a, grp, big, n_big, min_dp, min_iden, (uint32_t)end_clip, sub_out, huge, d.d_scal);
+	uint32_t n_huge = (uint32_t)d.get_scal(SC_AUX2);
+	if (n_huge) { // reads with more hits than a CTA can sort: device-wide sort of everything, keep only their rows
+		DSub *tmp = mab_alloc<DSub>(d, h.n_seq);
+		unsigned long long saved = d.get_scal(SC_COUNT);
+		dh_sub_global(d, h, min_dp, min_iden, end_clip, tmp, grp);
+		MAB_CUDA(cudaMemcpyAsync(d.d_scal + SC_COUNT, &saved, 8, cudaMemcpyHostToDevice, d.stream));
+		MAB_LAUNCH(d, k_sub_copy_listed, mab_grid(n_huge, 128), 128, 0, huge, n_huge, tmp, sub_out, d.d_scal + SC_COUNT);
+		d.sync();
+		d.free(tmp);
+	}
+	d.free(huge);
+}
+
 uint64_t dh_sub(MabDev &d, const DHits &h, int min_dp, float min_iden, int end_clip, DSub *sub_out)
 {
 	const uint32_t n_seq = h.n_seq;
@@ -771,23 +795,7 @@ uint64_t dh_sub(MabDev &d, const DHits &h, int min_dp, float min_iden, int end_c
 	static const int smem_sort = getenv("MAB_SUB_SMEM_SORT") && atoi(getenv("MAB_SUB_SMEM_SORT")) != 0; // 1: the shared-memory network
 	MAB_LAUNCH(d, k_sub_warp, grid, SUBW_WARPS * 32, 0, h.a, grp, n_seq, min_dp, min_iden, (uint32_t)end_clip, sub_out, big, d.d_scal, smem_sort);
 	uint32_t n_big = (uint32_t)d.get_scal(SC_BIG);
-	if (n_big) {
-		const size_t smem = (size_t)SUBC_HITS * 2 * 4;
-		MAB_CUDA(cudaFuncSetAttribute(k_sub_cta, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); // per device: set on every use
-		uint32_t *huge = mab_alloc<uint32_t>(d, n_big);
-		MAB_LAUNCH(d, k_sub_cta, n_big < MAB_SMS * 2 ? n_big : MAB_SMS * 2, 512, smem, h.a, grp, big, n_big, min_dp, min_iden, (uint32_t)end_clip, sub_out, huge, d.d_scal);
-		uint32_t n_huge = (uint32_t)d.get_scal(SC_AUX2);
-		if (n_huge) { // reads with more hits than a CTA can sort: device-wide sort of everything, keep only their rows
-			DSub *tmp = mab_alloc<DSub>(d, n_seq);
-			unsigned long long saved = d.get_scal(SC_COUNT);
-			dh_sub_global(d, h, min_dp, min_iden, end_clip, tmp, grp);
-			MAB_CUDA(cudaMemcpyAsync(d.d_scal + SC_COUNT, &saved, 8, cudaMemcpyHostToDevice, d.stream));
-			MAB_LAUNCH(d, k_sub_copy_listed, mab_grid(n_huge, 128), 128, 0, huge, n_huge, tmp, sub_out, d.d_scal + SC_COUNT);
-			d.sync();
-			d.free(tmp);
-		}
-		d.free(huge);
-	}
+	if (n_big) sub_big_reads(d, h, grp, big, n_big, min_dp, min_iden, end_clip, sub_out);
 	uint64_t n_remained = d.get_scal(SC_COUNT);
 	if (grp != h.grp) d.free(grp);
 	d.free(big);
@@ -805,7 +813,7 @@ static uint64_t dh_sub_global(MabDev &d, const DHits &h, int min_dp, float min_i
 	if (h.n >= (1ull << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 hits on one GPU\n"); exit(73); }
 	size_t nk = 2 * h.n;
 	uint64_t *ka = mab_alloc<uint64_t>(d, nk), *kb = mab_alloc<uint64_t>(d, nk);
-	MAB_LAUNCH(d, k_sub_keys, mab_grid(h.n, 256), 256, 0, h.a, h.n, min_iden, (uint32_t)end_clip, ka);
+	MAB_LAUNCH(d, k_sub_keys, mab_grid(h.n, 256), 256, 0, h.a, h.n, grp, min_iden, (uint32_t)end_clip, ka);
 	cub::DoubleBuffer<uint64_t> dk(ka, kb);
 	size_t tb = 0;
 	int end_bit = 33 + (int)bits_for(n_seq - 1);
@@ -1112,6 +1120,291 @@ size_t dh_contained(MabDev &d, DHits &h, DSub *sub, const uint8_t *seq_del, cons
 	if (cut_reg && ma_verbose_dev >= 3) fprintf(stderr, "[M::%s::%s] %ld hits remain after cut\n", "ma_hit_cut", sys_timestamp(), (long)gv[0]);
 	if (ma_verbose_dev >= 3)
 		fprintf(stderr, "[M::%s::%s] %d sequences and %ld hits remain after containment removal\n", "ma_hit_contained", sys_timestamp(), n_new, (long)gv[1]);
+	return h.n;
+}
+
+// ---------------------------------------------------------------------------------------------
+// dh_select: the default read selection as per-read passes over the sorted hit buckets.  Only the two cuts need another
+// read's interval (the target's) and only the renumbering needs every read's containment flag; everything else is local to
+// one query read.  So the hits stay in their buckets: each pass moves a read's surviving hits to the front of its bucket
+// (in order: survivors only move down, behind everything the warp has loaded) and shrinks the bound in h.grp.  Dead slots keep
+// their read's id.  A record is stored only when it moved or its cut changed it.  One final pass renumbers the survivors
+// and writes the dense, qid-ordered array the step functions would have left.
+// ---------------------------------------------------------------------------------------------
+enum { SCS_CUT = SC_TMP0, SCS_DP, SCS_LEN, SCS_FLT, SCS_CUT2, SCS_NSEQ, SCS_NHITS }; // d_scal slots of dh_select's counters
+
+__device__ __forceinline__ bool hit_clipped(const DHit &p, const DHit &o) { return p.qns != o.qns || p.qe != o.qe || p.ts != o.ts || p.te != o.te; }
+
+// ma_hit_cut + ma_hit_flt with sub1 (one sweep, as k_cut_flt), then ma_hit_sub with clip over the survivors (as k_sub_warp); one
+// warp per read.  Reads with more than SUBW_HITS survivors go to big_list for the CTA tier.  A read left without hits keeps
+// sub2 = {0,0}: ma_hit_sub never sees it.
+__global__ void __launch_bounds__(SUBW_WARPS * 32)
+k_sel_cut_flt_sub(DHit *a, uint64_t *grp, uint32_t n_seq, const DSub *__restrict__ sub1, int min_span, int max_hang, int min_ovlp,
+                  int min_dp, float min_iden, uint32_t clip, DSub *sub2, uint32_t *big_list, unsigned long long *scal)
+{
+	__shared__ uint32_t s_key[SUBW_WARPS][2 * SUBW_HITS];
+	__shared__ unsigned long long s_acc[3]; // per-read counters of the block (kept out of registers: the sort needs them)
+	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+	const unsigned lt = (1u << lane) - 1u;
+	uint32_t *key = s_key[warp];
+	unsigned long long dp = 0;
+	unsigned n_cut = 0;
+	if (threadIdx.x < 3) s_acc[threadIdx.x] = 0;
+	__syncthreads();
+	for (uint32_t r = blockIdx.x * SUBW_WARPS + warp; r < n_seq; r += gridDim.x * SUBW_WARPS) {
+		const uint64_t g = grp[r];
+		const uint32_t end = (uint32_t)g, first = (uint32_t)(g >> 32);
+		if (end == 0) continue;
+		const DSub sq = sub1[r];
+		uint32_t kept = 0, n = 0; // survivors and sub keys so far (uniform)
+		for (uint32_t c = first; c < end; c += 32) {
+			const uint32_t i = c + lane;
+			DHit p;
+			bool keep = false, dirty = false, key_ok = false;
+			uint32_t ks = 0, ke = 0;
+			if (i < end) {
+				p = ld_hit_rw(a + i);
+				const DHit o = p;
+				const DSub st = sub1[p.tn];
+				keep = mab_cut_hit(p, sq, st, min_span);
+				if (keep) {
+					++n_cut;
+					DArc t;
+					const uint32_t ql = sq.e - sq.s_del, tl = st.e - st.s_del;
+					const int rr = mab_hit2arc(p, (int)ql, (int)tl, max_hang, .5f, min_ovlp, &t);
+					keep = rr >= 0 || rr == MAB_HT_QCONT || rr == MAB_HT_TCONT;
+					if (keep) {
+						dp += rr >= 0 ? (uint32_t)rr : rr == MAB_HT_QCONT ? ql : tl;
+						dirty = hit_clipped(p, o);
+						key_ok = sub_hit_keys(p, r, min_iden, clip, &ks, &ke);
+					}
+				}
+			}
+			const unsigned km = __ballot_sync(0xffffffffu, keep);
+			const uint32_t dst = first + kept + __popc(km & lt);
+			if (keep && (dst != i || dirty)) st_hit(a + dst, p);
+			kept += __popc(km);
+			const unsigned sm = __ballot_sync(0xffffffffu, key_ok);
+			if (key_ok) { const uint32_t q = n + 2 * __popc(sm & lt); if (q < 2 * SUBW_HITS) key[q] = ks, key[q + 1] = ke; }
+			n += 2 * __popc(sm);
+		}
+		if (lane == 0) grp[r] = kept ? (uint64_t)first << 32 | (first + kept) : 0;
+		if (kept == 0) continue;
+		if (lane == 0) atomicAdd(&s_acc[0], (unsigned long long)(sq.e - (sq.s_del & 0x7fffffffu))), atomicAdd(&s_acc[1], (unsigned long long)kept);
+		if (kept > SUBW_HITS) { if (lane == 0) big_list[atomicAdd(scal + SC_BIG, 1ull)] = r; continue; }
+		uint32_t np = 32; while (np < n) np <<= 1;
+		__syncwarp();
+		switch (np) {
+			case 32: sub_sort_regs<1>(key, n, lane); break;
+			case 64: sub_sort_regs<2>(key, n, lane); break;
+			case 128: sub_sort_regs<4>(key, n, lane); break;
+			case 256: sub_sort_regs<8>(key, n, lane); break;
+			default: sub_sort_regs<16>(key, n, lane); break;
+		}
+		__syncwarp();
+		if (sub_sweep_smem(key, n, min_dp, clip, sub2 + r, lane) && lane == 0) atomicAdd(&s_acc[2], 1ull);
+		__syncwarp();
+	}
+	#pragma unroll
+	for (int o = 16; o; o >>= 1) dp += __shfl_xor_sync(0xffffffffu, dp, o);
+	n_cut = __reduce_add_sync(0xffffffffu, n_cut);
+	if (lane == 0) {
+		if (n_cut) atomicAdd(scal + SCS_CUT, (unsigned long long)n_cut);
+		if (dp) atomicAdd(scal + SCS_DP, dp);
+	}
+	__syncthreads();
+	if (threadIdx.x == 0) {
+		if (s_acc[0]) atomicAdd(scal + SCS_LEN, s_acc[0]);
+		if (s_acc[1]) atomicAdd(scal + SCS_FLT, s_acc[1]);
+		if (s_acc[2]) atomicAdd(scal + SC_COUNT, s_acc[2]);
+	}
+}
+
+// second ma_hit_cut with sub2 and the flag pass of ma_hit_contained against the merged table sub (as k_cut_cont_mark); one warp
+// per read.  tn_out[slot] = target of each surviving hit, for the count pass after the renumbering.
+__global__ void __launch_bounds__(256)
+k_sel_cut_cont(DHit *a, uint64_t *grp, uint32_t n_seq, const DSub *__restrict__ sub2, DSub *sub, int min_span, HitArcParams hp,
+               uint8_t *used, uint32_t *tn_out, unsigned long long *n_cut)
+{
+	const int lane = threadIdx.x & 31;
+	const unsigned lt = (1u << lane) - 1u;
+	unsigned cut = 0;
+	for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_seq; r += (gridDim.x * blockDim.x) >> 5) {
+		const uint64_t g = grp[r];
+		const uint32_t end = (uint32_t)g, first = (uint32_t)(g >> 32);
+		if (end == 0) continue;
+		const DSub rq = sub2[r];
+		uint32_t kept = 0;
+		for (uint32_t c = first; c < end; c += 32) {
+			const uint32_t i = c + lane;
+			DHit p;
+			bool keep = false, dirty = false;
+			if (i < end) {
+				p = ld_hit_rw(a + i);
+				const DHit o = p;
+				const DSub rt = sub2[p.tn];
+				keep = mab_cut_hit(p, rq, rt, min_span);
+				if (keep) {
+					dirty = hit_clipped(p, o);
+					DArc tmp;
+					const int rr = mab_hit2arc(p, (int)(rq.e - rq.s_del), (int)(rt.e - rt.s_del), hp.max_hang, hp.int_frac, hp.min_ovlp, &tmp);
+					if (rr == MAB_HT_QCONT) atomicOr(&sub[r].s_del, MAB_DEL_BIT);
+					else if (rr == MAB_HT_TCONT) atomicOr(&sub[p.tn].s_del, MAB_DEL_BIT);
+					used[p.tn] = 1;
+				}
+			}
+			const unsigned km = __ballot_sync(0xffffffffu, keep);
+			const uint32_t dst = first + kept + __popc(km & lt);
+			if (keep) {
+				if (dst != i || dirty) st_hit(a + dst, p);
+				tn_out[dst] = p.tn;
+			}
+			kept += __popc(km);
+		}
+		if (lane == 0) {
+			grp[r] = kept ? (uint64_t)first << 32 | (first + kept) : 0;
+			if (kept) used[r] = 1, cut += kept;
+		}
+	}
+	if (lane == 0 && cut) atomicAdd(n_cut, (unsigned long long)cut);
+}
+
+// hits of each kept read whose target is also kept, at the read's new id
+__global__ void __launch_bounds__(256)
+k_sel_final_count(const uint64_t *__restrict__ grp, const uint32_t *__restrict__ tn, const int32_t *__restrict__ map, uint32_t n_seq, uint32_t *cnt)
+{
+	const int lane = threadIdx.x & 31;
+	for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_seq; r += (gridDim.x * blockDim.x) >> 5) {
+		const int32_t m = map[r];
+		if (m < 0) continue;
+		const uint64_t g = grp[r];
+		const uint32_t end = (uint32_t)g, first = (uint32_t)(g >> 32);
+		unsigned c = 0;
+		if (end) for (uint32_t i = first + lane; i < end; i += 32) c += map[tn[i]] >= 0;
+		c = __reduce_add_sync(0xffffffffu, c);
+		if (lane == 0) cnt[m] = c;
+	}
+}
+
+// renumber the surviving hits of each kept read and write them densely at off[new id]; also reports the new read count
+// (*n_new) and hit count to scal
+__global__ void __launch_bounds__(256)
+k_sel_final_copy(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const int32_t *__restrict__ map, uint32_t n_seq,
+                 const uint32_t *__restrict__ off, const uint32_t *__restrict__ n_new, DHit *__restrict__ out, unsigned long long *scal)
+{
+	const int lane = threadIdx.x & 31;
+	const unsigned lt = (1u << lane) - 1u;
+	if (blockIdx.x == 0 && threadIdx.x == 0) { const uint32_t nn = *n_new; scal[SCS_NSEQ] = nn, scal[SCS_NHITS] = off[nn]; }
+	for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_seq; r += (gridDim.x * blockDim.x) >> 5) {
+		const int32_t m = map[r];
+		if (m < 0) continue;
+		const uint64_t g = grp[r];
+		const uint32_t end = (uint32_t)g, first = (uint32_t)(g >> 32);
+		if (end == 0) continue;
+		uint32_t o = off[m];
+		for (uint32_t c = first; c < end; c += 32) {
+			const uint32_t i = c + lane;
+			DHit h;
+			int32_t tn = -1;
+			if (i < end) { h = ld_hit(a + i); tn = map[h.tn]; }
+			const unsigned km = __ballot_sync(0xffffffffu, tn >= 0);
+			if (tn >= 0) {
+				h.qns = (uint64_t)(uint32_t)m << 32 | (uint32_t)h.qns, h.tn = (uint32_t)tn;
+				st_hit(out + o + __popc(km & lt), h);
+			}
+			o += __popc(km);
+		}
+	}
+}
+
+static unsigned warp_grid(uint32_t n_seq, unsigned warps_per_block)
+{
+	const unsigned g = (n_seq + warps_per_block - 1) / warps_per_block;
+	return g < 1 ? 1 : g < MAB_SMS * 32u ? g : MAB_SMS * 32u;
+}
+
+static void exclusive_sum(MabDev &d, const uint32_t *in, uint32_t *out, size_t n)
+{
+	size_t tb = 0;
+	cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, (int64_t)n, d.stream);
+	void *tmp = d.tmp(tb);
+	cub::DeviceScan::ExclusiveSum(tmp, tb, in, out, (int64_t)n, d.stream);
+	++d.n_lib;
+}
+
+size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t *map_out, float *cov, const std::function<void()> &step3)
+{
+	const uint32_t n_seq = h.n_seq;
+	if (h.n >= (1ull << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 hits on one GPU\n"); exit(73); }
+	if (!h.grp) { // hits that did not come through the sort (mab_load_hits): the bounds of their runs
+		h.grp = mab_alloc<uint64_t>(d, n_seq);
+		MAB_CUDA(cudaMemsetAsync(h.grp, 0, (size_t)n_seq * 8, d.stream));
+		if (h.n) MAB_LAUNCH(d, k_group_bounds, mab_grid(h.n, 256), 256, 0, h.a, h.n, (uint32_t*)h.grp);
+	}
+	dh_sub(d, h, o.min_dp, o.min_iden, 0, sub);
+	d.trace("select:sub1");
+
+	// ma_hit_cut + ma_hit_flt + ma_hit_sub (clip = min_span / 2)
+	const int clip = o.min_span / 2;
+	DSub *sub2 = mab_alloc<DSub>(d, n_seq);
+	uint32_t *big = mab_alloc<uint32_t>(d, n_seq);
+	MAB_CUDA(cudaMemsetAsync(sub2, 0, (size_t)n_seq * sizeof(DSub), d.stream));
+	d.zero_scal(0, SCS_NHITS + 1);
+	MAB_LAUNCH(d, k_sel_cut_flt_sub, warp_grid(n_seq, SUBW_WARPS), SUBW_WARPS * 32, 0, h.a, h.grp, n_seq, sub, o.min_span, o.flt_max_hang, o.flt_min_ovlp,
+	           o.min_dp, o.min_iden, (uint32_t)clip, sub2, big, d.d_scal);
+	const uint32_t n_big = (uint32_t)d.get_scal(SC_BIG);
+	{
+		unsigned long long gv[4] = { d.h_scal[SCS_DP], d.h_scal[SCS_LEN], d.h_scal[SCS_CUT], d.h_scal[SCS_FLT] };
+		sum_ranks(gv, 4);
+		*cov = (float)((double)gv[0] / gv[1]);
+		if (ma_verbose_dev >= 3) {
+			fprintf(stderr, "[M::%s::%s] %ld hits remain after cut\n", "ma_hit_cut", sys_timestamp(), (long)gv[2]);
+			fprintf(stderr, "[M::%s::%s] %ld hits remain after filtering; crude coverage after filtering: %.2f\n", "ma_hit_flt", sys_timestamp(), (long)gv[3], *cov);
+		}
+	}
+	step3();
+	if (n_big) sub_big_reads(d, h, h.grp, big, n_big, o.min_dp, o.min_iden, clip, sub2);
+	d.free(big);
+	{
+		unsigned long long v[1] = { d.get_scal(SC_COUNT) };
+		sum_ranks(v, 1);
+		if (ma_verbose_dev >= 3) fprintf(stderr, "[M::%s::%s] %ld query sequences remain after sub\n", "ma_hit_sub", sys_timestamp(), (long)v[0]);
+	}
+	dh_sub_merge(d, n_seq, sub, sub2);
+	d.trace("select:cut1+flt+sub2");
+
+	// ma_hit_cut with sub2 + ma_hit_contained's flags; h.a2 is idle until the final copy and holds the targets meanwhile
+	uint8_t *used = mab_alloc<uint8_t>(d, n_seq);
+	uint32_t *tn = reinterpret_cast<uint32_t*>(h.a2);
+	MAB_CUDA(cudaMemsetAsync(used, 0, n_seq, d.stream));
+	MAB_LAUNCH(d, k_sel_cut_cont, warp_grid(n_seq, 8), 256, 0, h.a, h.grp, n_seq, sub2, sub, o.min_span, o.cont, used, tn, d.d_scal + SCS_CUT2);
+
+	// renumbering: keep flags -> new ids (sub2 is dead and takes the compacted table), then hit counts -> offsets -> dense copy
+	uint32_t *keep = mab_alloc<uint32_t>(d, (size_t)n_seq + 1), *excl = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);
+	uint32_t *cnt = mab_alloc<uint32_t>(d, (size_t)n_seq + 1), *off = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);
+	MAB_CUDA(cudaMemsetAsync(keep + n_seq, 0, 4, d.stream));
+	MAB_LAUNCH(d, k_cont_keep, mab_grid(n_seq, 256), 256, 0, n_seq, sub, used, nullptr, keep);
+	exclusive_sum(d, keep, excl, (size_t)n_seq + 1);   // excl[n_seq] = reads kept
+	MAB_LAUNCH(d, k_cont_map, mab_grid(n_seq, 256), 256, 0, n_seq, keep, excl, map_out, sub, sub2);
+	MAB_LAUNCH(d, k_sel_final_count, warp_grid(n_seq, 8), 256, 0, h.grp, tn, map_out, n_seq, cnt); // cnt[0 ..< reads kept]
+	exclusive_sum(d, cnt, off, (size_t)n_seq + 1);      // off[reads kept] = hits kept; later entries are not used
+	MAB_LAUNCH(d, k_sel_final_copy, warp_grid(n_seq, 8), 256, 0, h.a, h.grp, map_out, n_seq, off, excl + n_seq, h.a2, d.d_scal);
+	const uint32_t n_new = (uint32_t)d.get_scal(SCS_NSEQ);
+	const size_t n_hits = (size_t)d.h_scal[SCS_NHITS];
+	const unsigned long long n_cut2 = d.h_scal[SCS_CUT2];
+	if (n_new) MAB_CUDA(cudaMemcpyAsync(sub, sub2, (size_t)n_new * sizeof(DSub), cudaMemcpyDeviceToDevice, d.stream));
+	d.free(sub2); d.free(used); d.free(keep); d.free(excl); d.free(cnt); d.free(off);
+	DHit *t = h.a; h.a = h.a2; h.a2 = t;
+	h.n = n_hits, h.n_seq = n_new;
+	drop_bounds(d, h);
+	d.trace("select:cut2+contained");
+
+	unsigned long long gv[2] = { n_cut2, (unsigned long long)h.n };
+	sum_ranks(gv, 2);
+	if (ma_verbose_dev >= 3) {
+		fprintf(stderr, "[M::%s::%s] %ld hits remain after cut\n", "ma_hit_cut", sys_timestamp(), (long)gv[0]);
+		fprintf(stderr, "[M::%s::%s] %d sequences and %ld hits remain after containment removal\n", "ma_hit_contained", sys_timestamp(), n_new, (long)gv[1]);
+	}
 	return h.n;
 }
 

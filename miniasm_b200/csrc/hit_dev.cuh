@@ -55,6 +55,13 @@ void dh_sub_merge(MabDev &d, uint32_t n_sub, DSub *a, const DSub *b);
 size_t dh_contained(MabDev &d, DHits &h, DSub *sub, const uint8_t *seq_del, const HitArcParams &p, int32_t *map_out,
                     const DSub *cut_reg = nullptr, int min_span = 0,
                     const std::function<void(DSub*, uint8_t*, uint32_t)> *exchange = nullptr);
+// The default read selection (main.c:119-142, -S 5 and up): ma_hit_sub, ma_hit_cut, ma_hit_flt, ma_hit_sub with end clipping,
+// ma_sub_merge, ma_hit_cut and ma_hit_contained, with the same results and [M::...] lines as calling the steps above in turn.
+// Runs as per-read passes over the hits' per-read buckets (h.grp; derived from the hits when null); step3() is called where
+// the second round begins (after the ma_hit_flt line).  sub: n_seq entries, the merged table compacted like dh_contained's.
+// Returns the new hit count; h.n_seq is the surviving read count and map_out[old] = new id or -1.
+struct SelectParams { int min_dp; float min_iden; int min_span; int flt_max_hang, flt_min_ovlp; HitArcParams cont; };
+size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t *map_out, float *cov, const std::function<void()> &step3);
 // ma_sg_gen without the final asg_cleanup: seq table + sorted local arcs (sharded runs clean up after exchanging seq flags)
 void dh_sg_emit(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g);
 // ma_hit_cut immediately followed by ma_hit_flt on the same table (main.c:123-125), fused
