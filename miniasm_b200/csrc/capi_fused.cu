@@ -117,6 +117,33 @@ static void ctx_reset_reads(mab_ctx *c)
 	c->n_seq = 0;
 }
 
+// a selection renumbered the reads (map[old] = new id or -1, c->hits.n_seq survivors): carry their original ids over
+static void renumber_reads(mab_ctx *c, const int32_t *map, uint32_t n_old)
+{
+	MabDev &d = c->dev;
+	uint32_t *orig_new = mab_alloc<uint32_t>(d, c->hits.n_seq);
+	if (n_old) MAB_LAUNCH(d, k_orig_from_map, mab_grid(n_old, 256), 256, 0, n_old, map, c->orig_id, orig_new);
+	d.free(c->orig_id);
+	c->orig_id = orig_new;
+	c->n_seq = c->hits.n_seq;
+}
+
+// the default read selection (both rounds, -S 5 and up) on the context's hits
+static void select_default(mab_ctx *c, const ma_opt_t *opt, const SelectHooks &hk)
+{
+	MabDev &d = c->dev;
+	const uint32_t n_old = c->n_seq;
+	d.free(c->sub);
+	c->sub = mab_alloc<DSub>(d, n_old);
+	d.trace("select:begin");
+	int32_t *map = mab_alloc<int32_t>(d, n_old);
+	const SelectParams sp = { opt->min_dp, opt->min_iden, opt->min_span, (int)(opt->max_hang * 1.5), (int)(opt->min_ovlp * .5),
+	                          { opt->max_hang, opt->int_frac, opt->min_ovlp } };
+	dh_select(d, c->hits, c->sub, sp, map, &c->cov, hk);
+	renumber_reads(c, map, n_old);
+	d.free(map);
+}
+
 extern "C" {
 
 mab_ctx_t *mab_create(int device)
@@ -328,25 +355,9 @@ int mab_select(mab_ctx_t *c, const ma_opt_t *opt, int no_first, int no_second, i
 	PhaseTimer pt(d, &c->stats.ms_select, "mab_select");
 	ctx_drop_graphs(c);
 	auto step3_banner = [] { if (!mab_mute && ma_verbose >= 1) fprintf(stderr, "[M::main] ===> Step 3: 2-pass (fine) read selection <===\n"); };
-	auto renumber = [c, &d](const int32_t *map, uint32_t n_old) {
-		uint32_t *orig_new = mab_alloc<uint32_t>(d, c->hits.n_seq);
-		if (n_old) MAB_LAUNCH(d, k_orig_from_map, mab_grid(n_old, 256), 256, 0, n_old, map, c->orig_id, orig_new);
-		d.free(c->orig_id);
-		c->orig_id = orig_new;
-		c->n_seq = c->hits.n_seq;
-	};
 	if (!no_first && !no_second && stage >= 5) { // the whole selection: per-read passes over the hit buckets
 		if (!mab_mute && ma_verbose >= 1) fprintf(stderr, "[M::main] ===> Step 2: 1-pass (crude) read selection <===\n");
-		d.free(c->sub);
-		c->sub = mab_alloc<DSub>(d, c->n_seq);
-		d.trace("select:begin");
-		const uint32_t n_old = c->n_seq;
-		int32_t *map = mab_alloc<int32_t>(d, n_old);
-		const SelectParams sp = { opt->min_dp, opt->min_iden, opt->min_span, (int)(opt->max_hang * 1.5), (int)(opt->min_ovlp * .5),
-		                          { opt->max_hang, opt->int_frac, opt->min_ovlp } };
-		dh_select(d, h, c->sub, sp, map, &c->cov, step3_banner);
-		renumber(map, n_old);
-		d.free(map);
+		select_default(c, opt, { step3_banner });
 		c->stats.n_hits_final = h.n, c->stats.n_seq_final = c->n_seq;
 		d.sync();
 		return 0;
@@ -359,8 +370,8 @@ int mab_select(mab_ctx_t *c, const ma_opt_t *opt, int no_first, int no_second, i
 			d.trace("select:begin");
 			dh_sub(d, h, opt->min_dp, opt->min_iden, 0, c->sub);
 			d.trace("select:sub1");
-			if (stage >= 3) dh_cut_flt(d, h, c->sub, opt->min_span, (int)(opt->max_hang * 1.5), (int)(opt->min_ovlp * .5), &c->cov);
-			else dh_cut(d, h, c->sub, opt->min_span);
+			dh_cut(d, h, c->sub, opt->min_span);
+			if (stage >= 3) dh_flt(d, h, c->sub, (int)(opt->max_hang * 1.5), (int)(opt->min_ovlp * .5), &c->cov);
 			d.trace("select:cut1(+flt)");
 		}
 	}
@@ -380,7 +391,7 @@ int mab_select(mab_ctx_t *c, const ma_opt_t *opt, int no_first, int no_second, i
 			int32_t *map = mab_alloc<int32_t>(d, n_old);
 			HitArcParams p = { opt->max_hang, opt->int_frac, opt->min_ovlp };
 			dh_contained(d, h, c->sub, nullptr, p, map);
-			renumber(map, n_old);
+			renumber_reads(c, map, n_old);
 			d.free(map);
 			d.trace("select:contained");
 		}
@@ -772,12 +783,12 @@ static void sum_over_ranks(void *ctx, unsigned long long *v, int n) // MabCountH
 	d.free(buf);
 }
 
-/* default read selection (main.c:119-142 with no -1/-2/-S): the interval tables are completed by all-reduce */
+/* default read selection (main.c:119-142 with no -1/-2/-S): dh_select on this rank's hits, with the per-rank interval tables
+ * and containment flags completed by all-reduce between its passes */
 int mab_select_sharded(mab_ctx_t *c, const ma_opt_t *opt)
 {
 	MAB_CUDA(cudaSetDevice(c->dev.device));
 	MabDev &d = c->dev;
-	DHits &h = c->hits;
 	ShardComm &sc = c->sc;
 	PhaseTimer pt(d, &c->stats.ms_select, "mab_select_sharded");
 	ctx_drop_graphs(c);
@@ -785,40 +796,17 @@ int mab_select_sharded(mab_ctx_t *c, const ma_opt_t *opt)
 	if (sc.rank != 0) mab_mute = 1; // only rank 0 talks (thread-local: ranks may be threads of one process); the counts it prints are summed over the ranks
 	mab_count_hook = sum_over_ranks, mab_count_hook_ctx = c;
 	const uint32_t n = c->n_seq;
-	d.free(c->sub);
-	c->sub = mab_alloc<DSub>(d, n);
-	d.trace("shard-select:begin");
-	dh_sub(d, h, opt->min_dp, opt->min_iden, 0, c->sub);                  // rows of the reads this rank owns; zeros elsewhere
-	d.trace("shard-select:sub1");
-	sc_allreduce(d, sc, c->sub, n, ncclUint64, ncclSum);                   // every row is written by exactly one rank
-	d.trace("shard-select:all-reduce sub1");
-	dh_cut_flt(d, h, c->sub, opt->min_span, (int)(opt->max_hang * 1.5), (int)(opt->min_ovlp * .5), &c->cov);
-	d.trace("shard-select:cut1+flt");
-	DSub *sub2 = mab_alloc<DSub>(d, n), *cut2 = mab_alloc<DSub>(d, n);
-	dh_sub(d, h, opt->min_dp, opt->min_iden, opt->min_span / 2, sub2);
-	d.trace("shard-select:sub2");
-	sc_allreduce(d, sc, sub2, n, ncclUint64, ncclSum);
-	if (n) MAB_CUDA(cudaMemcpyAsync(cut2, sub2, (size_t)n * sizeof(DSub), cudaMemcpyDeviceToDevice, d.stream));
-	dh_sub_merge(d, n, c->sub, sub2);
-	d.free(sub2);
-	int32_t *map = mab_alloc<int32_t>(d, n);
-	HitArcParams p = { opt->max_hang, opt->int_frac, opt->min_ovlp };
-	std::function<void(DSub*, uint8_t*, uint32_t)> ex = [&](DSub *sub, uint8_t *used, uint32_t n_seq) {
+	SelectHooks hk;
+	hk.sub_done = [&](DSub *s) { sc_allreduce(d, sc, s, n, ncclUint64, ncclSum); }; // a row is written by the rank owning the read only
+	hk.flags_done = [&](DSub *sub, uint8_t *used, uint32_t n_seq) {
 		// containment flags are the top bit of the first word: an element-wise max over ranks is their OR (the other bits agree)
 		sc_allreduce(d, sc, sub, (size_t)n_seq * 2, ncclUint32, ncclMax);
 		sc_allreduce(d, sc, used, n_seq, ncclUint8, ncclMax);
 	};
-	dh_contained(d, h, c->sub, nullptr, p, map, cut2, opt->min_span, &ex);
-	d.trace("shard-select:cut2+contained (+2 all-reduces)");
-	uint32_t *orig_new = mab_alloc<uint32_t>(d, h.n_seq);
-	if (n) MAB_LAUNCH(d, k_orig_from_map, mab_grid(n, 256), 256, 0, n, map, c->orig_id, orig_new);
-	d.free(c->orig_id);
-	c->orig_id = orig_new;
-	c->n_seq = h.n_seq;
-	d.free(map); d.free(cut2);
+	select_default(c, opt, hk);
 	mab_mute = msave;
 	mab_count_hook = nullptr, mab_count_hook_ctx = nullptr;
-	c->stats.n_hits_final = h.n, c->stats.n_seq_final = c->n_seq;
+	c->stats.n_hits_final = c->hits.n, c->stats.n_seq_final = c->n_seq;
 	d.sync();
 	return 0;
 }

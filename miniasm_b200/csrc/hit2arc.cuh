@@ -80,3 +80,15 @@ __host__ __device__ __forceinline__ bool mab_cut_hit(DHit &p, const DSub rq, con
 		return keep;
 	}
 }
+
+// ma_hit_flt (hit.c:195-216): true if hit h of query interval sq / target interval st classifies as an arc or a containment under
+// the (already relaxed) thresholds; *dp is then what it adds to the numerator of the coverage estimate the reference logs
+__host__ __device__ __forceinline__ bool mab_flt_hit(const DHit &h, const DSub sq, const DSub st, int max_hang, int min_ovlp, uint32_t *dp)
+{
+	if ((sq.s_del | st.s_del) & MAB_DEL_BIT) return false;
+	const uint32_t ql = sq.e - sq.s_del, tl = st.e - st.s_del;
+	DArc t;
+	const int r = mab_hit2arc(h, (int)ql, (int)tl, max_hang, .5f, min_ovlp, &t);
+	*dp = r >= 0 ? (uint32_t)r : r == MAB_HT_QCONT ? ql : tl;
+	return r >= 0 || r == MAB_HT_QCONT || r == MAB_HT_TCONT;
+}

@@ -66,7 +66,6 @@ void dh_free(MabDev &d, DHits &h)
 // generic library selection, so the hit path has its own three-step compaction -- per-tile keep counts
 // (flags only), a scan of the ~n/2048 tile counts, and a scatter in which every warp row reads 1 KB of contiguous
 // records and writes them behind the tile's offset.  Order of the kept hits is the input order.
-// MAB_CUB_SELECT=1 switches back to cub::DeviceSelect::Flagged.
 // ---------------------------------------------------------------------------------------------
 constexpr int SEL_ROWS = 8, SEL_THREADS = 256, SEL_TILE = SEL_ROWS * SEL_THREADS;
 static_assert(SEL_ROWS * (SEL_THREADS / 32) == 64, "k_sel_scatter scans exactly two counts per lane of one warp");
@@ -137,31 +136,23 @@ k_sel_scatter(const DHit *__restrict__ in, const uint8_t *__restrict__ flag, siz
 static size_t select_hits(MabDev &d, DHits &h, const uint8_t *flag)
 {
 	if (h.n == 0) return 0;
-	static const bool use_cub = getenv("MAB_CUB_SELECT") && atoi(getenv("MAB_CUB_SELECT")) != 0;
+	if (h.n >= (1ull << 32)) { fprintf(stderr, "[E::miniasm_b200] more than 2^32 hits on one GPU\n"); exit(73); }
 	unsigned long long *d_n = d.d_scal + SC_NSEL;
-	if (use_cub || h.n >= (1ull << 32)) {
-		size_t tb = 0;
-		cub::DeviceSelect::Flagged(nullptr, tb, h.a, flag, h.a2, d_n, (int64_t)h.n, d.stream);
-		void *tmp = d.tmp(tb);
-		cub::DeviceSelect::Flagged(tmp, tb, h.a, flag, h.a2, d_n, (int64_t)h.n, d.stream);
-		++d.n_lib;
-	} else {
-		const uint32_t n_tile = (uint32_t)((h.n + SEL_TILE - 1) / SEL_TILE);
-		uint32_t *cnt = mab_alloc<uint32_t>(d, n_tile), *off = mab_alloc<uint32_t>(d, n_tile);
-		d.zero_scal(SC_NSEL);
-		MAB_LAUNCH(d, k_sel_count, n_tile, SEL_THREADS, 0, flag, h.n, cnt, d_n);
-		if ((size_t)d.get_scal(SC_NSEL) == h.n) { // every record stays (clean data: the common case of ma_hit_cut/flt): nothing to move
-			d.free(cnt); d.free(off);
-			return h.n;
-		}
-		size_t tb = 0;
-		cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt, off, (int)n_tile, d.stream);
-		void *tmp = d.tmp(tb);
-		cub::DeviceScan::ExclusiveSum(tmp, tb, cnt, off, (int)n_tile, d.stream);
-		++d.n_lib;
-		MAB_LAUNCH(d, k_sel_scatter, n_tile, SEL_THREADS, 0, h.a, flag, h.n, off, h.a2, d_n);
-		d.free(cnt); d.free(off);   // stream-ordered arena: reuse is ordered behind the kernels above
+	const uint32_t n_tile = (uint32_t)((h.n + SEL_TILE - 1) / SEL_TILE);
+	uint32_t *cnt = mab_alloc<uint32_t>(d, n_tile), *off = mab_alloc<uint32_t>(d, n_tile);
+	d.zero_scal(SC_NSEL);
+	MAB_LAUNCH(d, k_sel_count, n_tile, SEL_THREADS, 0, flag, h.n, cnt, d_n);
+	if ((size_t)d.get_scal(SC_NSEL) == h.n) { // every record stays (clean data: the common case of ma_hit_cut/flt): nothing to move
+		d.free(cnt); d.free(off);
+		return h.n;
 	}
+	size_t tb = 0;
+	cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt, off, (int)n_tile, d.stream);
+	void *tmp = d.tmp(tb);
+	cub::DeviceScan::ExclusiveSum(tmp, tb, cnt, off, (int)n_tile, d.stream);
+	++d.n_lib;
+	MAB_LAUNCH(d, k_sel_scatter, n_tile, SEL_THREADS, 0, h.a, flag, h.n, off, h.a2, d_n);
+	d.free(cnt); d.free(off);   // stream-ordered arena: reuse is ordered behind the kernels above
 	size_t n = (size_t)d.get_scal(SC_NSEL);
 	DHit *t = h.a; h.a = h.a2; h.a2 = t;
 	h.n = n;
@@ -467,7 +458,7 @@ k_sub_sweep(const uint64_t *key, const uint64_t *grp, uint32_t n_seq, int min_dp
 
 // ---- shared-memory variant: one warp (<= SUBW_HITS hits) or one CTA (<= SUBC_HITS hits) per read ------------
 // The endpoints of one read never leave the SM: load the group's hits (two 128-bit loads each), emit the keys into
-// shared memory, bitonic-sort them there, sweep the depth with the same warp scan as k_sub_sweep.  Only reads
+// shared memory, sort them (the warp in registers), sweep the depth with the same warp scan as k_sub_sweep.  Only reads
 // with more hits than a CTA can hold go through the device-wide sort above.
 constexpr int SUBW_WARPS = 8;
 constexpr int SUBW_HITS = 256;               // per warp: 512 keys = 2 KB
@@ -543,7 +534,7 @@ __device__ __forceinline__ void sub_sort_regs(uint32_t *key, const uint32_t n, c
 
 __global__ void __launch_bounds__(SUBW_WARPS * 32)
 k_sub_warp(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, uint32_t n_seq, int min_dp, float min_iden, uint32_t clip,
-           DSub *sub, uint32_t *big_list, unsigned long long *scal, int smem_sort)
+           DSub *sub, uint32_t *big_list, unsigned long long *scal)
 {
 	__shared__ uint32_t s_key[SUBW_WARPS][2 * SUBW_HITS];
 	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -566,34 +557,14 @@ k_sub_warp(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, uint32_
 		}
 		uint32_t np = 32; while (np < n) np <<= 1;
 		__syncwarp();
-		if (!smem_sort) { // keys of the read sorted in registers (np is uniform across the warp)
-			switch (np) {
-				case 32: sub_sort_regs<1>(key, n, lane); break;
-				case 64: sub_sort_regs<2>(key, n, lane); break;
-				case 128: sub_sort_regs<4>(key, n, lane); break;
-				case 256: sub_sort_regs<8>(key, n, lane); break;
-				default: sub_sort_regs<16>(key, n, lane); break;
-			}
-			__syncwarp();
-			remained += sub_sweep_smem(key, n, min_dp, clip, sub + r, lane);
-			__syncwarp();
-			continue;
+		switch (np) { // keys of the read sorted in registers (np is uniform across the warp)
+			case 32: sub_sort_regs<1>(key, n, lane); break;
+			case 64: sub_sort_regs<2>(key, n, lane); break;
+			case 128: sub_sort_regs<4>(key, n, lane); break;
+			case 256: sub_sort_regs<8>(key, n, lane); break;
+			default: sub_sort_regs<16>(key, n, lane); break;
 		}
-		for (uint32_t i = n + lane; i < np; i += 32) key[i] = 0xffffffffu;
 		__syncwarp();
-		// bitonic network; j = 1 << lj is a power of two, so the pair index comes from shifts (a 32-bit division per
-		// compare-exchange made this loop most of the kernel's instructions)
-		for (uint32_t k = 2, lk = 1; k <= np; k <<= 1, ++lk)
-			for (uint32_t lj = lk; lj-- > 0;) {
-				const uint32_t j = 1u << lj;
-				for (uint32_t t = lane; t < np / 2; t += 32) {
-					const uint32_t lo = ((t >> lj) << (lj + 1)) | (t & (j - 1)), hi = lo + j;
-					const uint32_t x = key[lo], y = key[hi];
-					const bool asc = (lo & k) == 0;
-					if ((x > y) == asc) key[lo] = y, key[hi] = x;
-				}
-				__syncwarp();
-			}
 		remained += sub_sweep_smem(key, n, min_dp, clip, sub + r, lane);
 		__syncwarp();
 	}
@@ -779,27 +750,28 @@ static void sub_big_reads(MabDev &d, const DHits &h, const uint64_t *grp, const 
 uint64_t dh_sub(MabDev &d, const DHits &h, int min_dp, float min_iden, int end_clip, DSub *sub_out)
 {
 	const uint32_t n_seq = h.n_seq;
+	unsigned long long n_remained = 0;
 	if (n_seq) MAB_CUDA(cudaMemsetAsync(sub_out, 0, (size_t)n_seq * sizeof(DSub), d.stream));
-	if (h.n == 0 || n_seq == 0) return 0;
-	if (h.n >= (1ull << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 hits on one GPU\n"); exit(73); }
-	uint64_t *grp = h.grp;              // the bounds the sort left, while no pass has moved the hits since
-	if (!grp) {
-		grp = mab_alloc<uint64_t>(d, n_seq);
-		MAB_CUDA(cudaMemsetAsync(grp, 0, (size_t)n_seq * 8, d.stream));
-		MAB_LAUNCH(d, k_group_bounds, mab_grid(h.n, 256), 256, 0, h.a, h.n, (uint32_t*)grp);
+	if (h.n && n_seq) {
+		if (h.n >= (1ull << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 hits on one GPU\n"); exit(73); }
+		uint64_t *grp = h.grp;              // the bounds the sort left, while no pass has moved the hits since
+		if (!grp) {
+			grp = mab_alloc<uint64_t>(d, n_seq);
+			MAB_CUDA(cudaMemsetAsync(grp, 0, (size_t)n_seq * 8, d.stream));
+			MAB_LAUNCH(d, k_group_bounds, mab_grid(h.n, 256), 256, 0, h.a, h.n, (uint32_t*)grp);
+		}
+		uint32_t *big = mab_alloc<uint32_t>(d, n_seq);
+		MAB_CUDA(cudaMemsetAsync(d.d_scal, 0, 8 * sizeof(unsigned long long), d.stream));
+		unsigned grid = (n_seq + SUBW_WARPS - 1) / SUBW_WARPS;
+		if (grid > MAB_SMS * 32u) grid = MAB_SMS * 32u;
+		MAB_LAUNCH(d, k_sub_warp, grid, SUBW_WARPS * 32, 0, h.a, grp, n_seq, min_dp, min_iden, (uint32_t)end_clip, sub_out, big, d.d_scal);
+		uint32_t n_big = (uint32_t)d.get_scal(SC_BIG);
+		if (n_big) sub_big_reads(d, h, grp, big, n_big, min_dp, min_iden, end_clip, sub_out);
+		n_remained = d.get_scal(SC_COUNT);
+		if (grp != h.grp) d.free(grp);
+		d.free(big);
 	}
-	uint32_t *big = mab_alloc<uint32_t>(d, n_seq);
-	MAB_CUDA(cudaMemsetAsync(d.d_scal, 0, 8 * sizeof(unsigned long long), d.stream));
-	unsigned grid = (n_seq + SUBW_WARPS - 1) / SUBW_WARPS;
-	if (grid > MAB_SMS * 32u) grid = MAB_SMS * 32u;
-	static const int smem_sort = getenv("MAB_SUB_SMEM_SORT") && atoi(getenv("MAB_SUB_SMEM_SORT")) != 0; // 1: the shared-memory network
-	MAB_LAUNCH(d, k_sub_warp, grid, SUBW_WARPS * 32, 0, h.a, grp, n_seq, min_dp, min_iden, (uint32_t)end_clip, sub_out, big, d.d_scal, smem_sort);
-	uint32_t n_big = (uint32_t)d.get_scal(SC_BIG);
-	if (n_big) sub_big_reads(d, h, grp, big, n_big, min_dp, min_iden, end_clip, sub_out);
-	uint64_t n_remained = d.get_scal(SC_COUNT);
-	if (grp != h.grp) d.free(grp);
-	d.free(big);
-	{ unsigned long long v[1] = { n_remained }; sum_ranks(v, 1); n_remained = v[0]; }
+	sum_ranks(&n_remained, 1);          // a collective: every rank gets here, with or without hits
 	if (ma_verbose_dev >= 3)
 		fprintf(stderr, "[M::%s::%s] %ld query sequences remain after sub\n", "ma_hit_sub", sys_timestamp(), (long)n_remained);
 	return n_remained;
@@ -840,99 +812,6 @@ __global__ void k_cut(DHit *a, size_t n, const DSub *__restrict__ reg, int min_s
 	}
 }
 
-// ma_hit_cut followed by ma_hit_flt on the same interval table (main.c:123-125) in one sweep and one compaction
-__global__ void k_cut_flt(DHit *a, size_t n, const DSub *__restrict__ sub, int min_span, int max_hang, int min_ovlp, uint8_t *flag,
-                          unsigned long long *n_cut, unsigned long long *tot_dp)
-{
-	unsigned long long dp = 0;
-	unsigned cut = 0;
-	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-		DHit p = ld_hit_rw(a + i);
-		const DSub sq = sub[p.qns >> 32], st = sub[p.tn];
-		bool keep = mab_cut_hit(p, sq, st, min_span);
-		if (keep) {
-			++cut;
-			DArc t;
-			const uint32_t ql = sq.e - sq.s_del, tl = st.e - st.s_del;
-			const int r = mab_hit2arc(p, (int)ql, (int)tl, max_hang, .5f, min_ovlp, &t);
-			keep = r >= 0 || r == MAB_HT_QCONT || r == MAB_HT_TCONT;
-			if (keep) { dp += r >= 0 ? (uint32_t)r : r == MAB_HT_QCONT ? ql : tl; st_hit(a + i, p); }
-		}
-		flag[i] = keep;
-	}
-	typedef cub::BlockReduce<unsigned long long, 256> BR;
-	__shared__ typename BR::TempStorage ts;
-	unsigned long long s = BR(ts).Sum(dp);
-	__syncthreads();
-	unsigned long long c = BR(ts).Sum((unsigned long long)cut);
-	if (threadIdx.x == 0) { if (s) atomicAdd(tot_dp, s); if (c) atomicAdd(n_cut, c); }
-}
-
-// second-round ma_hit_cut fused with pass 1 of ma_hit_contained (hit.c:231-236): clip, then classify the clipped hit
-// against the merged interval table (its lengths equal those of the round-2 table) and raise containment flags
-__global__ void k_cut_cont_mark(DHit *a, size_t n, const DSub *__restrict__ sub2, DSub *sub, int min_span, HitArcParams hp,
-                                uint8_t *used, uint8_t *flag, unsigned long long *n_cut)
-{
-	unsigned cut = 0;
-	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-		DHit p = ld_hit_rw(a + i);
-		const uint32_t q = (uint32_t)(p.qns >> 32), t = p.tn;
-		const DSub rq = sub2[q], rt = sub2[t];
-		const bool keep = mab_cut_hit(p, rq, rt, min_span);
-		if (keep) {
-			++cut;
-			st_hit(a + i, p);
-			DArc tmp;
-			const int r = mab_hit2arc(p, (int)(rq.e - rq.s_del), (int)(rt.e - rt.s_del), hp.max_hang, hp.int_frac, hp.min_ovlp, &tmp);
-			if (r == MAB_HT_QCONT) atomicOr(&sub[q].s_del, MAB_DEL_BIT);
-			else if (r == MAB_HT_TCONT) atomicOr(&sub[t].s_del, MAB_DEL_BIT);
-			used[q] = 1, used[t] = 1;
-		}
-		flag[i] = keep;
-	}
-	cut = __reduce_add_sync(0xffffffffu, cut);
-	if ((threadIdx.x & 31) == 0 && cut) atomicAdd(n_cut, (unsigned long long)cut);
-}
-
-__global__ void k_cont_apply2(DHit *a, size_t n, const int32_t *__restrict__ map, uint8_t *flag)
-{
-	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-		bool keep = flag[i];
-		if (keep) {
-			uint64_t qns = a[i].qns;
-			int32_t qn = map[qns >> 32], tn = map[a[i].tn];
-			keep = qn >= 0 && tn >= 0;
-			if (keep) { a[i].qns = (uint64_t)(uint32_t)qn << 32 | (uint32_t)qns; a[i].tn = (uint32_t)tn; }
-		}
-		flag[i] = keep;
-	}
-}
-
-__global__ void k_flt_len(const DHit *a, size_t n, const DSub *__restrict__ sub, unsigned long long *tot_len);
-
-size_t dh_cut_flt(MabDev &d, DHits &h, const DSub *sub, int min_span, int max_hang, int min_ovlp, float *cov)
-{
-	unsigned long long tot_dp = 0, tot_len = 0, n_cut = 0;
-	if (h.n) {
-		uint8_t *flag = mab_alloc<uint8_t>(d, h.n);
-		d.zero_scal(SC_AUX, 2);
-		d.zero_scal(SC_COUNT, 1);
-		MAB_LAUNCH(d, k_cut_flt, mab_grid(h.n, 256), 256, 0, h.a, h.n, sub, min_span, max_hang, min_ovlp, flag, d.d_scal + SC_COUNT, d.d_scal + SC_AUX);
-		select_hits(d, h, flag);
-		d.free(flag);
-		if (h.n) MAB_LAUNCH(d, k_flt_len, mab_grid(h.n, 256), 256, 0, h.a, h.n, sub, d.d_scal + SC_AUX2);
-		tot_dp = d.get_scal(SC_AUX), tot_len = d.h_scal[SC_AUX2], n_cut = d.h_scal[SC_COUNT];
-	}
-	unsigned long long gv[4] = { tot_dp, tot_len, n_cut, (unsigned long long)h.n };
-	sum_ranks(gv, 4);
-	*cov = (float)((double)gv[0] / gv[1]);
-	if (ma_verbose_dev >= 3) {
-		fprintf(stderr, "[M::%s::%s] %ld hits remain after cut\n", "ma_hit_cut", sys_timestamp(), (long)gv[2]);
-		fprintf(stderr, "[M::%s::%s] %ld hits remain after filtering; crude coverage after filtering: %.2f\n", "ma_hit_flt", sys_timestamp(), (long)gv[3], *cov);
-	}
-	return h.n;
-}
-
 size_t dh_cut(MabDev &d, DHits &h, const DSub *reg, int min_span)
 {
 	if (h.n) {
@@ -954,17 +833,9 @@ __global__ void k_flt(const DHit *a, size_t n, const DSub *__restrict__ sub, int
 	unsigned long long dp = 0;
 	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
 		DHit h = ld_hit(a + i);
-		const DSub sq = sub[h.qns >> 32], st = sub[h.tn];
-		bool keep = false;
-		if (!((sq.s_del | st.s_del) & MAB_DEL_BIT)) {
-			DArc t;
-			const uint32_t ql = sq.e - sq.s_del, tl = st.e - st.s_del;
-			int r = mab_hit2arc(h, (int)ql, (int)tl, max_hang, .5f, min_ovlp, &t);
-			if (r >= 0 || r == MAB_HT_QCONT || r == MAB_HT_TCONT) {
-				keep = true;
-				dp += r >= 0 ? (uint32_t)r : r == MAB_HT_QCONT ? ql : tl;
-			}
-		}
+		uint32_t l;
+		const bool keep = mab_flt_hit(h, sub[h.qns >> 32], sub[h.tn], max_hang, min_ovlp, &l);
+		if (keep) dp += l;
 		flag[i] = keep;
 	}
 	typedef cub::BlockReduce<unsigned long long, 256> BR;
@@ -1068,25 +939,16 @@ __global__ void k_cont_apply(DHit *a, size_t n, const int32_t *__restrict__ map,
 	}
 }
 
-size_t dh_contained(MabDev &d, DHits &h, DSub *sub, const uint8_t *seq_del, const HitArcParams &p, int32_t *map_out, const DSub *cut_reg, int min_span,
-                    const std::function<void(DSub*, uint8_t*, uint32_t)> *exchange)
+size_t dh_contained(MabDev &d, DHits &h, DSub *sub, const uint8_t *seq_del, const HitArcParams &p, int32_t *map_out)
 {
 	const uint32_t n_seq = h.n_seq;
 	uint32_t n_new = 0;
-	unsigned long long n_cut = 0;
-	uint8_t *cut_flag = nullptr;
 	if (n_seq) {
 		uint8_t *used = mab_alloc<uint8_t>(d, n_seq);
 		uint32_t *keep = mab_alloc<uint32_t>(d, n_seq), *excl = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);
 		DSub *sub2 = mab_alloc<DSub>(d, n_seq);
 		MAB_CUDA(cudaMemsetAsync(used, 0, n_seq, d.stream));
-		if (cut_reg && h.n) { // fused with the preceding ma_hit_cut: one sweep clips and classifies, one compaction at the end
-			cut_flag = mab_alloc<uint8_t>(d, h.n);
-			d.zero_scal(SC_COUNT, 1);
-			MAB_LAUNCH(d, k_cut_cont_mark, mab_grid(h.n, 256), 256, 0, h.a, h.n, cut_reg, sub, min_span, p, used, cut_flag, d.d_scal + SC_COUNT);
-		} else
 		if (h.n) MAB_LAUNCH(d, k_cont_mark, mab_grid(h.n, 256), 256, 0, h.a, h.n, sub, p, used);
-		if (exchange) (*exchange)(sub, used, n_seq); // sharded runs: OR the containment flags and the "used" marks of all ranks
 		MAB_LAUNCH(d, k_cont_keep, mab_grid(n_seq, 256), 256, 0, n_seq, sub, used, seq_del, keep);
 		size_t tb = 0;
 		cub::DeviceScan::ExclusiveSum(nullptr, tb, keep, excl, (int)n_seq, d.stream);
@@ -1100,12 +962,7 @@ size_t dh_contained(MabDev &d, DHits &h, DSub *sub, const uint8_t *seq_del, cons
 		d.sync();
 		n_new = last_keep + last_excl;
 		if (n_new) MAB_CUDA(cudaMemcpyAsync(sub, sub2, (size_t)n_new * sizeof(DSub), cudaMemcpyDeviceToDevice, d.stream));
-		if (cut_flag) {
-			n_cut = d.get_scal(SC_COUNT);
-			MAB_LAUNCH(d, k_cont_apply2, mab_grid(h.n, 256), 256, 0, h.a, h.n, map_out, cut_flag);
-			select_hits(d, h, cut_flag);
-			d.free(cut_flag);
-		} else if (h.n) {
+		if (h.n) {
 			uint8_t *flag = mab_alloc<uint8_t>(d, h.n);
 			MAB_LAUNCH(d, k_cont_apply, mab_grid(h.n, 256), 256, 0, h.a, h.n, map_out, flag);
 			select_hits(d, h, flag);
@@ -1115,11 +972,10 @@ size_t dh_contained(MabDev &d, DHits &h, DSub *sub, const uint8_t *seq_del, cons
 	}
 	h.n_seq = n_new;
 	drop_bounds(d, h);                  // reads renumbered
-	unsigned long long gv[2] = { (unsigned long long)n_cut, (unsigned long long)h.n };
-	sum_ranks(gv, 2);
-	if (cut_reg && ma_verbose_dev >= 3) fprintf(stderr, "[M::%s::%s] %ld hits remain after cut\n", "ma_hit_cut", sys_timestamp(), (long)gv[0]);
+	unsigned long long n_hits = h.n;
+	sum_ranks(&n_hits, 1);
 	if (ma_verbose_dev >= 3)
-		fprintf(stderr, "[M::%s::%s] %d sequences and %ld hits remain after containment removal\n", "ma_hit_contained", sys_timestamp(), n_new, (long)gv[1]);
+		fprintf(stderr, "[M::%s::%s] %d sequences and %ld hits remain after containment removal\n", "ma_hit_contained", sys_timestamp(), n_new, (long)n_hits);
 	return h.n;
 }
 
@@ -1135,7 +991,7 @@ enum { SCS_CUT = SC_TMP0, SCS_DP, SCS_LEN, SCS_FLT, SCS_CUT2, SCS_NSEQ, SCS_NHIT
 
 __device__ __forceinline__ bool hit_clipped(const DHit &p, const DHit &o) { return p.qns != o.qns || p.qe != o.qe || p.ts != o.ts || p.te != o.te; }
 
-// ma_hit_cut + ma_hit_flt with sub1 (one sweep, as k_cut_flt), then ma_hit_sub with clip over the survivors (as k_sub_warp); one
+// ma_hit_cut + ma_hit_flt with sub1 in one sweep, then ma_hit_sub with clip over the survivors (as k_sub_warp); one
 // warp per read.  Reads with more than SUBW_HITS survivors go to big_list for the CTA tier.  A read left without hits keeps
 // sub2 = {0,0}: ma_hit_sub never sees it.
 __global__ void __launch_bounds__(SUBW_WARPS * 32)
@@ -1169,12 +1025,10 @@ k_sel_cut_flt_sub(DHit *a, uint64_t *grp, uint32_t n_seq, const DSub *__restrict
 				keep = mab_cut_hit(p, sq, st, min_span);
 				if (keep) {
 					++n_cut;
-					DArc t;
-					const uint32_t ql = sq.e - sq.s_del, tl = st.e - st.s_del;
-					const int rr = mab_hit2arc(p, (int)ql, (int)tl, max_hang, .5f, min_ovlp, &t);
-					keep = rr >= 0 || rr == MAB_HT_QCONT || rr == MAB_HT_TCONT;
+					uint32_t l;
+					keep = mab_flt_hit(p, sq, st, max_hang, min_ovlp, &l);
 					if (keep) {
-						dp += rr >= 0 ? (uint32_t)rr : rr == MAB_HT_QCONT ? ql : tl;
+						dp += l;
 						dirty = hit_clipped(p, o);
 						key_ok = sub_hit_keys(p, r, min_iden, clip, &ks, &ke);
 					}
@@ -1220,8 +1074,9 @@ k_sel_cut_flt_sub(DHit *a, uint64_t *grp, uint32_t n_seq, const DSub *__restrict
 	}
 }
 
-// second ma_hit_cut with sub2 and the flag pass of ma_hit_contained against the merged table sub (as k_cut_cont_mark); one warp
-// per read.  tn_out[slot] = target of each surviving hit, for the count pass after the renumbering.
+// second ma_hit_cut with sub2, then the flag pass of ma_hit_contained (as k_cont_mark) on the clipped hit: lengths from sub2 (the
+// merged table's are the same), flags raised in the merged table sub; one warp per read.  tn_out[slot] = target of each surviving
+// hit, for the count pass after the renumbering.
 __global__ void __launch_bounds__(256)
 k_sel_cut_cont(DHit *a, uint64_t *grp, uint32_t n_seq, const DSub *__restrict__ sub2, DSub *sub, int min_span, HitArcParams hp,
                uint8_t *used, uint32_t *tn_out, unsigned long long *n_cut)
@@ -1332,7 +1187,7 @@ static void exclusive_sum(MabDev &d, const uint32_t *in, uint32_t *out, size_t n
 	++d.n_lib;
 }
 
-size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t *map_out, float *cov, const std::function<void()> &step3)
+size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t *map_out, float *cov, const SelectHooks &hk)
 {
 	const uint32_t n_seq = h.n_seq;
 	if (h.n >= (1ull << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 hits on one GPU\n"); exit(73); }
@@ -1342,6 +1197,7 @@ size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t 
 		if (h.n) MAB_LAUNCH(d, k_group_bounds, mab_grid(h.n, 256), 256, 0, h.a, h.n, (uint32_t*)h.grp);
 	}
 	dh_sub(d, h, o.min_dp, o.min_iden, 0, sub);
+	if (hk.sub_done) hk.sub_done(sub);
 	d.trace("select:sub1");
 
 	// ma_hit_cut + ma_hit_flt + ma_hit_sub (clip = min_span / 2)
@@ -1362,7 +1218,7 @@ size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t 
 			fprintf(stderr, "[M::%s::%s] %ld hits remain after filtering; crude coverage after filtering: %.2f\n", "ma_hit_flt", sys_timestamp(), (long)gv[3], *cov);
 		}
 	}
-	step3();
+	if (hk.step3) hk.step3();
 	if (n_big) sub_big_reads(d, h, h.grp, big, n_big, o.min_dp, o.min_iden, clip, sub2);
 	d.free(big);
 	{
@@ -1370,6 +1226,7 @@ size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t 
 		sum_ranks(v, 1);
 		if (ma_verbose_dev >= 3) fprintf(stderr, "[M::%s::%s] %ld query sequences remain after sub\n", "ma_hit_sub", sys_timestamp(), (long)v[0]);
 	}
+	if (hk.sub_done) hk.sub_done(sub2);
 	dh_sub_merge(d, n_seq, sub, sub2);
 	d.trace("select:cut1+flt+sub2");
 
@@ -1378,6 +1235,7 @@ size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t 
 	uint32_t *tn = reinterpret_cast<uint32_t*>(h.a2);
 	MAB_CUDA(cudaMemsetAsync(used, 0, n_seq, d.stream));
 	MAB_LAUNCH(d, k_sel_cut_cont, warp_grid(n_seq, 8), 256, 0, h.a, h.grp, n_seq, sub2, sub, o.min_span, o.cont, used, tn, d.d_scal + SCS_CUT2);
+	if (hk.flags_done) hk.flags_done(sub, used, n_seq);
 
 	// renumbering: keep flags -> new ids (sub2 is dead and takes the compacted table), then hit counts -> offsets -> dense copy
 	uint32_t *keep = mab_alloc<uint32_t>(d, (size_t)n_seq + 1), *excl = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);

@@ -50,22 +50,24 @@ void dh_sub_merge(MabDev &d, uint32_t n_sub, DSub *a, const DSub *b);
 // (sdict.c:69-86).  seq_del: per-read deletion flags of the dictionary on entry (may be null = none).
 // On return sub is compacted in place, hits renumbered/compacted, map_out[old] = new id or -1, and
 // h.n_seq is the surviving read count.  Returns the new hit count.
-// With cut_reg != null the call first applies ma_hit_cut(cut_reg, min_span) to the hits (fused sweep, one compaction).
-// `exchange` (sharded runs) is called between the flag pass and the renumbering with (sub, used, n_seq).
-size_t dh_contained(MabDev &d, DHits &h, DSub *sub, const uint8_t *seq_del, const HitArcParams &p, int32_t *map_out,
-                    const DSub *cut_reg = nullptr, int min_span = 0,
-                    const std::function<void(DSub*, uint8_t*, uint32_t)> *exchange = nullptr);
+size_t dh_contained(MabDev &d, DHits &h, DSub *sub, const uint8_t *seq_del, const HitArcParams &p, int32_t *map_out);
 // The default read selection (main.c:119-142, -S 5 and up): ma_hit_sub, ma_hit_cut, ma_hit_flt, ma_hit_sub with end clipping,
 // ma_sub_merge, ma_hit_cut and ma_hit_contained, with the same results and [M::...] lines as calling the steps above in turn.
-// Runs as per-read passes over the hits' per-read buckets (h.grp; derived from the hits when null); step3() is called where
-// the second round begins (after the ma_hit_flt line).  sub: n_seq entries, the merged table compacted like dh_contained's.
-// Returns the new hit count; h.n_seq is the surviving read count and map_out[old] = new id or -1.
+// Runs as per-read passes over the hits' per-read buckets (h.grp; derived from the hits when null).  sub: n_seq entries, the
+// merged table compacted like dh_contained's.  Returns the new hit count; h.n_seq is the surviving read count and
+// map_out[old] = new id or -1.
 struct SelectParams { int min_dp; float min_iden; int min_span; int flt_max_hang, flt_min_ovlp; HitArcParams cont; };
-size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t *map_out, float *cov, const std::function<void()> &step3);
+// Callbacks of dh_select; an empty member is skipped.  step3: where the second round begins (after the ma_hit_flt line).
+// sub_done(table): after each ma_hit_sub, with the n_seq rows it wrote.  flags_done(sub, used, n_seq): after the containment
+// flags and "used" marks are raised, before the renumbering reads them.  A sharded run completes its per-rank rows there.
+struct SelectHooks {
+	std::function<void()> step3;
+	std::function<void(DSub*)> sub_done;
+	std::function<void(DSub*, uint8_t*, uint32_t)> flags_done;
+};
+size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t *map_out, float *cov, const SelectHooks &hk);
 // ma_sg_gen without the final asg_cleanup: seq table + sorted local arcs (sharded runs clean up after exchanging seq flags)
 void dh_sg_emit(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g);
-// ma_hit_cut immediately followed by ma_hit_flt on the same table (main.c:123-125), fused
-size_t dh_cut_flt(MabDev &d, DHits &h, const DSub *sub, int min_span, int max_hang, int min_ovlp, float *cov);
 
 // ma_sg_gen (asm.c:9-39): lens/del per read -> graph with arcs emitted in hit order, then asg_cleanup.
 void dh_sg_gen(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g);

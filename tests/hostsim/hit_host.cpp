@@ -1,8 +1,9 @@
-// hit_host.cpp -- TEST INFRASTRUCTURE (never linked into the product): the two functions that carry the reference's integer
-// conversion rules -- mab_cut_hit (ma_hit_cut's clipping, hit.c:162-193) and mab_hit2arc (miniasm.h:86-104), both in
-// miniasm_b200/csrc/hit2arc.cuh, the very header the CUDA kernels are built from -- compiled for the host and put behind the
-// loops of ma_hit_cut / ma_hit_flt / ma_sg_gen, so that the CPU tier can fuzz them against the unmodified reference with inputs
-// no synthetic PAF produces (hits reaching outside the kept intervals, wrapped spans, empty intervals, self hits):
+// hit_host.cpp -- TEST INFRASTRUCTURE (never linked into the product): the functions that carry the reference's integer
+// conversion rules -- mab_cut_hit (ma_hit_cut's clipping, hit.c:162-193), mab_flt_hit (ma_hit_flt's keep rule, hit.c:195-216)
+// and mab_hit2arc (miniasm.h:86-104), all in miniasm_b200/csrc/hit2arc.cuh, the very header the CUDA kernels are built from --
+// compiled for the host and put behind the loops of ma_hit_cut / ma_hit_flt / ma_sg_gen, so that the CPU tier can fuzz them
+// against the unmodified reference with inputs no synthetic PAF produces (hits reaching outside the kept intervals, wrapped spans,
+// empty intervals, self hits):
 // tests/test_hitrules_cpu.py.  Also here: mab_comp_of (basecomp.cuh), the reverse-strand complement of `-f reads`, all 256 byte values.
 #include "../../miniasm_b200/csrc/hit2arc.cuh"
 #include "../../miniasm_b200/csrc/basecomp.cuh"
@@ -20,20 +21,15 @@ size_t hs_hit_cut(const DSub *reg, int min_span, size_t n, DHit *a)
 	return m;
 }
 
-// ma_hit_flt (hit.c:195-216): keep what classifies as an arc or a containment under the (already relaxed) thresholds;
-// *tot_dp is the numerator of the coverage estimate the reference logs
+// ma_hit_flt (hit.c:195-216): stable in-place compaction by mab_flt_hit; *tot_dp is the numerator of the coverage estimate
 size_t hs_hit_flt(const DSub *sub, int max_hang, int min_ovlp, size_t n, DHit *a, unsigned long long *tot_dp)
 {
 	size_t m = 0;
 	unsigned long long dp = 0;
 	for (size_t i = 0; i < n; ++i) {
 		const DHit h = a[i];
-		const DSub sq = sub[h.qns >> 32], st = sub[h.tn];
-		if ((sq.s_del | st.s_del) & MAB_DEL_BIT) continue;
-		const uint32_t ql = sq.e - sq.s_del, tl = st.e - st.s_del;
-		DArc t;
-		const int r = mab_hit2arc(h, (int)ql, (int)tl, max_hang, .5f, min_ovlp, &t);
-		if (r >= 0 || r == MAB_HT_QCONT || r == MAB_HT_TCONT) a[m++] = h, dp += r >= 0 ? (uint32_t)r : r == MAB_HT_QCONT ? ql : tl;
+		uint32_t l;
+		if (mab_flt_hit(h, sub[h.qns >> 32], sub[h.tn], max_hang, min_ovlp, &l)) a[m++] = h, dp += l;
 	}
 	*tot_dp = dp;
 	return m;

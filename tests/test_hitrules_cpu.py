@@ -1,5 +1,5 @@
-"""CPU tier: the integer-conversion rules of ma_hit_cut (hit.c:162-193) and ma_hit2arc (miniasm.h:86-104) as the CUDA kernels
-compile them (miniasm_b200/csrc/hit2arc.cuh, built for the host by tests/hostsim/hit_host.cpp), fuzzed against the unmodified
+"""CPU tier: the integer-conversion rules of ma_hit_cut (hit.c:162-193), ma_hit_flt's keep rule (hit.c:195-216) and ma_hit2arc
+(miniasm.h:86-104) as the CUDA kernels compile them (miniasm_b200/csrc/hit2arc.cuh, built for the host by tests/hostsim/hit_host.cpp), fuzzed against the unmodified
 reference with hits no synthetic PAF produces: ends outside the kept intervals, wrapped spans (qe < qs), empty and deleted
 intervals, self hits, palindromic self hits, every threshold from tiny to huge (SURVEY.md section 7 "hard part 2": which
 comparisons are signed and which unsigned is part of the behaviour)."""

@@ -1,8 +1,10 @@
 """The default read selection (mab_select with stage 100) runs as per-read passes over the hit buckets.  Its results must be
 exactly what the oracle port's step functions give: the merged interval table, the surviving hits in order (del bit masked),
 names, read and hit counts, and the [M::ma_hit_*] counters printed at verbose 3.  Inputs: the synthetic sets, and a hand-made
-file whose reads sit on both sides of every tier limit after filtering and that has hits dropped by each step."""
+file whose reads sit on both sides of every tier limit after filtering and that has hits dropped by each step, and an empty
+file.  The sharded selection (mab_select_sharded) runs the same passes and is held to the same results with one rank."""
 import ctypes as C
+import math
 import re
 
 import numpy as np
@@ -60,11 +62,18 @@ def write_tiers_paf(path):
 def pafs(paf_dir):
     out = {name: synth.generate(name, f"{paf_dir}/{name}.paf") for name in SETS}
     out["tiers"] = write_tiers_paf(f"{paf_dir}/tiers.paf")
+    out["empty"] = f"{paf_dir}/empty.paf"
+    open(out["empty"], "w").close()
     return out
 
 
 def n_kept(sub):
     return int(((sub["s_del"] & DEL) == 0).sum() - ((sub["s_del"] == 0) & (sub["e"] == 0)).sum())
+
+
+def c_2f(x):
+    """printf's %.2f, which keeps the sign of a NaN (the coverage of an empty input is 0 / 0)"""
+    return f"{x:.2f}" if x == x else "-nan" if math.copysign(1.0, x) < 0 else "nan"
 
 
 def port_select(port, paf):
@@ -76,7 +85,7 @@ def port_select(port, paf):
     p.cut()
     lines.append(f"ma_hit_cut: {p.n_hits} hits remain after cut")
     p.flt()
-    lines.append(f"ma_hit_flt: {p.n_hits} hits remain after filtering; crude coverage after filtering: {p.cov.value:.2f}")
+    lines.append(f"ma_hit_flt: {p.n_hits} hits remain after filtering; crude coverage after filtering: {c_2f(p.cov.value)}")
     s2 = port.ma_hit_sub(o.min_dp, o.min_iden, o.min_span // 2, p.n_hits, p.hits, n_seq)
     lines.append(f"ma_hit_sub: {n_kept(capi.np_from_ptr(s2, n_seq, SUB_DT))} query sequences remain after sub")
     capi.c_free(s2)
@@ -94,21 +103,30 @@ def counter_lines(err):
     return [f"{m.group(1)}: {m.group(2)}" for m in re.finditer(r"^\[M::(ma_hit_\w+)::[^\]]*\] (.*)$", err, re.M)]
 
 
-def fused_select(prod, port, paf, capfd, from_hits):
+def fused_select(prod, port, paf, capfd, how):
+    """how: "ingest" (the single-GPU path), "hits" (hits handed over without the sort's per-read bounds) or "sharded" (the
+    sharded ingest and selection with one rank: the collectives have nothing to combine)."""
     opt = prod.default_opt()
     ctx = prod.mab_create(0)
-    if from_hits:   # hits handed over without the sort's per-read bounds
+    if how == "hits":
         p = Pipeline(port, paf).read()
         assert prod.mab_load_hits(ctx, p.hits, p.n_hits, p.d) == 0
         p.free()
     else:
         data = open(paf, "rb").read()
         assert prod.mab_load_paf_text(ctx, data, len(data)) == 0
-        prod.mab_ingest(ctx, opt.min_span, opt.min_match, 1)
+        if how == "sharded":
+            assert prod.mab_shard_init(ctx, 0, 1, None) == 0
+            prod.mab_ingest_sharded(ctx, opt.min_span, opt.min_match, 1)
+        else:
+            prod.mab_ingest(ctx, opt.min_span, opt.min_match, 1)
     capfd.readouterr()
     prod.set_verbose(3)
     try:
-        prod.mab_select(ctx, C.byref(opt), 0, 0, 100)
+        if how == "sharded":
+            prod.mab_select_sharded(ctx, C.byref(opt))
+        else:
+            prod.mab_select(ctx, C.byref(opt), 0, 0, 100)
         prod.mab_sync(ctx)
     finally:
         prod.set_verbose(0)
@@ -132,14 +150,19 @@ def check(got, want):
     assert len(got["hits"]) == len(want["hits"]) and np.array_equal(got["hits"], want["hits"])
 
 
-@pytest.mark.parametrize("name", SETS + ["tiers"])
+@pytest.mark.parametrize("name", SETS + ["tiers", "empty"])
 def test_select_matches_port(name, pafs, port, prod, capfd):
-    check(fused_select(prod, port, pafs[name], capfd, False), port_select(port, pafs[name]))
+    check(fused_select(prod, port, pafs[name], capfd, "ingest"), port_select(port, pafs[name]))
 
 
 @pytest.mark.parametrize("name", ["chaos", "skew_small", "tiers"])
 def test_select_from_loaded_hits(name, pafs, port, prod, capfd):
-    check(fused_select(prod, port, pafs[name], capfd, True), port_select(port, pafs[name]))
+    check(fused_select(prod, port, pafs[name], capfd, "hits"), port_select(port, pafs[name]))
+
+
+@pytest.mark.parametrize("name", SETS + ["tiers"])
+def test_select_sharded_matches_port(name, pafs, port, prod, capfd):
+    check(fused_select(prod, port, pafs[name], capfd, "sharded"), port_select(port, pafs[name]))
 
 
 def test_tiers_paf_reaches_every_case(pafs, port):

@@ -32,8 +32,8 @@ SETS = {
 # "multi": jitter 30 on 10 kb reads makes equal-length arcs out of one unitig end common; the order of the L lines of such
 # ties is the order the reference's unstable in-place radix sort happens to leave (DESIGN.md "Tie order")
 TIES = {"multi"}
-SWITCHES = [{}, {"MAB_CUB_SELECT": "1"}, {"MAB_SUB_SMEM_SORT": "1"}, {"MAB_GPU_GFA": "0", "MAB_WRITER_THREADS": "3"}, {"MAB_GPU_GFA": "0"},
-            {"MAB_SG_SEGSORT": "0"}, {"MAB_CUB_SELECT": "1", "MAB_SUB_SMEM_SORT": "1", "MAB_GPU_GFA": "0", "MAB_SG_SEGSORT": "0"}]
+SWITCHES = [{}, {"MAB_GPU_GFA": "0", "MAB_WRITER_THREADS": "3"}, {"MAB_GPU_GFA": "0"}, {"MAB_SG_SEGSORT": "0"},
+            {"MAB_GPU_GFA": "0", "MAB_SG_SEGSORT": "0"}]
 
 
 @pytest.fixture(scope="module")
