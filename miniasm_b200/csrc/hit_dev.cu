@@ -196,16 +196,36 @@ __device__ __forceinline__ void warp_bitonic_regs(T (&v)[M], const int lane)
 
 // ---------------------------------------------------------------------------------------------
 // ma_hit_sort as a per-read bucket sort.  The number of reads is known and each read has ~100 hits, so the query-id part of
-// the key is a counting sort (per-read counts -> exclusive scan -> every hit's key scattered into its read's bucket with an
-// atomic cursor) and the query-start part a small sort per bucket.  A bucket holds key = qs << 32 | input position in the
-// nondeterministic order of the cursor; the keys are unique, so sorting them gives exactly the stable order by (qid, qs).
-// Three tiers by bucket size: a warp sorts up to BKW_HITS keys in registers, a CTA up to BKC_HITS with a block merge sort
-// (skewed sets: ~10 000 hits on each read of a hot locus), and larger buckets go to a segmented device sort of their keys only.
-// The sorted records land in h.a2 (then swapped with h.a); the bucket bounds become h.grp for ma_hit_sub.
+// the key is a counting sort (per-read counts -> exclusive scan -> every record scattered into its read's bucket with an
+// atomic cursor) and the query-start part a small sort per bucket.  Inside a bucket every record has the same query id, so that
+// half of qns carries an ordinal instead: a number that grows with the hit's input position (the position itself, or
+// 2 * line + 1 for a mirrored hit in the fused ingest).  key = qs << 32 | ordinal is unique in its bucket, so sorting by it gives
+// exactly the stable order by (qid, qs); the query id is written back when the sorted record is stored.
+// Three tiers by bucket size, all reading h.a2's buckets and writing the sorted records to the same positions of h.a: a warp
+// stages up to BKW_HITS records in shared memory and sorts (key, slot) pairs in registers; a CTA sorts up to BKC_HITS keys with
+// a block merge sort (skewed sets: ~10 000 hits on each read of a hot locus) and stores every record at its key's rank; larger
+// buckets go to a segmented device sort of their (key, slot) pairs, then a gather inside each bucket.  The bucket bounds become
+// h.grp for ma_hit_sub.
 // ---------------------------------------------------------------------------------------------
-constexpr int BKW_WARPS = 8, BKW_HITS = 256;
+constexpr int BKW_WARPS = 4, BKW_HITS = 256;
 constexpr int BKC_THREADS = 512, BKC_ITEMS = 32, BKC_HITS = BKC_THREADS * BKC_ITEMS;
 typedef unsigned long long BKey;
+
+// first 8 bytes of a bucket slot: qs, ordinal
+__device__ __forceinline__ BKey bucket_key(uint2 w) { return (BKey)w.x << 32 | w.y; }
+
+// the record of a bucket slot stored at dst as a hit of read q
+__device__ __forceinline__ void bucket_put(DHit *dst, uint4 x, uint4 y, uint32_t q)
+{
+	x.y = q;
+	uint4 *o = reinterpret_cast<uint4*>(dst);
+	o[0] = x, o[1] = y;
+}
+__device__ __forceinline__ void bucket_put(DHit *dst, const DHit *src, uint32_t q)
+{
+	const uint4 *s = reinterpret_cast<const uint4*>(src);
+	bucket_put(dst, __ldg(s), __ldg(s + 1), q);
+}
 
 __global__ void k_bucket_count(const DHit *a, size_t n, uint32_t *cnt)
 {
@@ -213,82 +233,160 @@ __global__ void k_bucket_count(const DHit *a, size_t n, uint32_t *cnt)
 		atomicAdd(&cnt[a[i].qns >> 32], 1u);
 }
 
-__global__ void k_bucket_fill(const DHit *a, size_t n, const uint32_t *__restrict__ first, uint32_t *cur, BKey *key)
+// every record into its read's bucket, with its input position as the ordinal
+__global__ void k_bucket_fill(const DHit *__restrict__ a, size_t n, const uint32_t *__restrict__ first, uint32_t *cur, DHit *__restrict__ out)
 {
 	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-		const uint64_t qns = a[i].qns;
-		const uint32_t q = (uint32_t)(qns >> 32);
-		key[first[q] + atomicAdd(&cur[q], 1u)] = (BKey)(uint32_t)qns << 32 | i;
+		const uint4 *p = reinterpret_cast<const uint4*>(a + i);
+		uint4 x = __ldg(p);
+		const uint4 y = __ldg(p + 1);
+		const uint32_t q = x.y;
+		x.y = (uint32_t)i;
+		uint4 *o = reinterpret_cast<uint4*>(out + first[q] + atomicAdd(&cur[q], 1u));
+		o[0] = x, o[1] = y;
 	}
 }
 
+// warp_bitonic_regs with a payload carried along each key.  The keys are distinct except the padding (~0), whose payloads
+// may be duplicated and are never read.
 template <int M>
-__device__ __forceinline__ void bucket_sort_regs(const DHit *__restrict__ a, const BKey *__restrict__ key, uint32_t f, uint32_t cnt, DHit *__restrict__ out, int lane)
+__device__ __forceinline__ void warp_bitonic_pairs(BKey (&v)[M], uint32_t (&p)[M], const int lane)
+{
+	#pragma unroll
+	for (int k = 2; k <= 32 * M; k <<= 1) {
+		#pragma unroll
+		for (int j = k >> 1; j > 0; j >>= 1) {
+			if (j >= 32) {
+				#pragma unroll
+				for (int m = 0; m < M; ++m) {
+					const int pm = m ^ (j >> 5);
+					if (pm > m) {
+						const bool asc = ((32 * m) & k) == 0; // k >= 64 here: the lane bits do not reach it
+						if ((v[pm] < v[m]) == asc) {
+							const BKey t = v[m]; v[m] = v[pm], v[pm] = t;
+							const uint32_t u = p[m]; p[m] = p[pm], p[pm] = u;
+						}
+					}
+				}
+			} else {
+				const bool low = (lane & j) == 0;
+				#pragma unroll
+				for (int m = 0; m < M; ++m) {
+					const BKey y = __shfl_xor_sync(0xffffffffu, v[m], j);
+					const uint32_t py = __shfl_xor_sync(0xffffffffu, p[m], j);
+					const bool asc = ((32 * m + lane) & k) == 0;
+					if ((asc == low) != (v[m] < y)) v[m] = y, p[m] = py;
+				}
+			}
+		}
+	}
+}
+
+// s = the bucket's cnt records staged in shared memory (two uint4 per record)
+template <int M>
+__device__ __forceinline__ void bucket_sort_regs(const uint4 *s, uint32_t cnt, uint32_t q, DHit *__restrict__ out, int lane)
 {
 	BKey v[M];
+	uint32_t p[M];
 	#pragma unroll
-	for (int m = 0; m < M; ++m) v[m] = 32u * m + lane < cnt ? key[f + 32 * m + lane] : ~0ull;
-	warp_bitonic_regs<M>(v, lane);
+	for (int m = 0; m < M; ++m) {
+		const uint32_t j = 32u * m + lane;
+		v[m] = j < cnt ? bucket_key(*reinterpret_cast<const uint2*>(s + 2 * j)) : ~0ull, p[m] = j;
+	}
+	warp_bitonic_pairs<M>(v, p, lane);
 	#pragma unroll
-	for (int m = 0; m < M; ++m)
-		if (32u * m + lane < cnt) st_hit(out + f + 32 * m + lane, ld_hit(a + (uint32_t)v[m]));
+	for (int m = 0; m < M; ++m) {
+		const uint32_t j = 32u * m + lane;
+		if (j < cnt) bucket_put(out + j, s[2 * p[m]], s[2 * p[m] + 1], q);
+	}
 }
 
 __global__ void __launch_bounds__(BKW_WARPS * 32)
-k_bucket_warp(const DHit *__restrict__ a, const BKey *__restrict__ key, const uint32_t *__restrict__ first, uint32_t n_seq,
+k_bucket_warp(const DHit *__restrict__ a, const uint32_t *__restrict__ first, uint32_t n_seq,
               DHit *__restrict__ out, uint64_t *grp, uint32_t *big_list, unsigned long long *scal)
 {
+	__shared__ uint4 s_rec[BKW_WARPS][2 * BKW_HITS]; // one bucket's records per warp
 	const int lane = threadIdx.x & 31;
+	uint4 *s = s_rec[threadIdx.x >> 5];
 	for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_seq; r += (gridDim.x * blockDim.x) >> 5) {
 		const uint32_t f = first[r], e = first[r + 1], cnt = e - f;
 		if (lane == 0) grp[r] = cnt ? (uint64_t)f << 32 | e : 0;
 		if (cnt == 0) continue;
 		if (cnt > BKW_HITS) { if (lane == 0) big_list[atomicAdd(scal + SC_BIG, 1ull)] = r; continue; }
-		if (cnt <= 32) bucket_sort_regs<1>(a, key, f, cnt, out, lane);
-		else if (cnt <= 64) bucket_sort_regs<2>(a, key, f, cnt, out, lane);
-		else if (cnt <= 128) bucket_sort_regs<4>(a, key, f, cnt, out, lane);
-		else bucket_sort_regs<8>(a, key, f, cnt, out, lane);
+		const uint4 *src = reinterpret_cast<const uint4*>(a + f);
+		for (uint32_t u = lane; u < 2 * cnt; u += 32) s[u] = __ldg(src + u);
+		__syncwarp();
+		if (cnt <= 32) bucket_sort_regs<1>(s, cnt, r, out + f, lane);
+		else if (cnt <= 64) bucket_sort_regs<2>(s, cnt, r, out + f, lane);
+		else if (cnt <= 128) bucket_sort_regs<4>(s, cnt, r, out + f, lane);
+		else bucket_sort_regs<8>(s, cnt, r, out + f, lane);
+		__syncwarp(); // the next bucket overwrites the staged records
 	}
 }
 
 struct BKeyLess { __device__ __forceinline__ bool operator()(const BKey &x, const BKey &y) const { return x < y; } };
 typedef cub::BlockMergeSort<BKey, BKC_THREADS, BKC_ITEMS> BkcSort;
+static_assert(sizeof(typename BkcSort::TempStorage) >= BKC_HITS * sizeof(BKey), "the sorted keys reuse the sort's storage");
 
+// The keys are sorted alone (a slot payload would not fit the registers of 16 384 keys per CTA); the sorted keys then go to
+// shared memory and every record finds its rank there by binary search: the keys are unique, so it finds exactly its own.
 __global__ void __launch_bounds__(BKC_THREADS, 1)
-k_bucket_cta(const DHit *__restrict__ a, const BKey *__restrict__ key, const uint32_t *__restrict__ first, const uint32_t *__restrict__ big_list,
+k_bucket_cta(const DHit *__restrict__ a, const uint32_t *__restrict__ first, const uint32_t *__restrict__ big_list,
              uint32_t n_big, DHit *__restrict__ out, uint32_t *huge_list, unsigned long long *scal)
 {
 	extern __shared__ __align__(16) unsigned char bk_smem[];
 	typename BkcSort::TempStorage &ts = *reinterpret_cast<typename BkcSort::TempStorage*>(bk_smem);
+	BKey *s_key = reinterpret_cast<BKey*>(bk_smem);
 	const uint32_t tid = threadIdx.x;
 	for (uint32_t b = blockIdx.x; b < n_big; b += gridDim.x) {
 		const uint32_t r = big_list[b], f = first[r], cnt = first[r + 1] - f;
 		if (cnt > BKC_HITS) { if (tid == 0) huge_list[atomicAdd(scal + SC_AUX2, 1ull)] = r; continue; }
 		BKey v[BKC_ITEMS];
 		#pragma unroll
-		for (int k = 0; k < BKC_ITEMS; ++k) { const uint32_t j = k * BKC_THREADS + tid; v[k] = j < cnt ? key[f + j] : ~0ull; } // padding sorts last
-		BkcSort(ts).Sort(v, BKeyLess());
-		#pragma unroll
-		for (int k = 0; k < BKC_ITEMS; ++k) { // blocked: thread tid holds ranks tid * BKC_ITEMS + k
-			const uint32_t j = tid * BKC_ITEMS + k;
-			if (j < cnt) st_hit(out + f + j, ld_hit(a + (uint32_t)v[k]));
+		for (int k = 0; k < BKC_ITEMS; ++k) { // padding sorts last
+			const uint32_t j = k * BKC_THREADS + tid;
+			v[k] = j < cnt ? bucket_key(__ldg(reinterpret_cast<const uint2*>(a + f + j))) : ~0ull;
 		}
-		__syncthreads(); // the temp storage is reused by the next bucket
+		BkcSort(ts).Sort(v, BKeyLess());
+		__syncthreads(); // the sort's storage becomes the sorted key array
+		#pragma unroll
+		for (int k = 0; k < BKC_ITEMS; ++k) s_key[tid * BKC_ITEMS + k] = v[k]; // blocked: thread tid holds ranks tid * BKC_ITEMS + k
+		__syncthreads();
+		for (uint32_t j = tid; j < cnt; j += BKC_THREADS) {
+			const uint4 *src = reinterpret_cast<const uint4*>(a + f + j);
+			const uint4 x = __ldg(src), y = __ldg(src + 1);
+			const BKey key = bucket_key(make_uint2(x.x, x.y));
+			uint32_t lo = 0, n = cnt; // last rank whose key is <= key
+			while (n > 1) { const uint32_t half = n >> 1; lo = s_key[lo + half] <= key ? lo + half : lo; n -= half; }
+			bucket_put(out + f + lo, x, y, r);
+		}
+		__syncthreads(); // the storage is reused by the next bucket
 	}
 }
 
-__global__ void k_bucket_segs(const uint32_t *list, uint32_t n, const uint32_t *first, int *beg, int *end)
+// Buckets beyond a CTA: their (key, slot) pairs are laid out bucket after bucket at off[b] (exclusive scan of the sizes).
+__global__ void k_bucket_sizes(const uint32_t *list, uint32_t n, const uint32_t *first, uint32_t *sz)
 {
-	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
-		beg[i] = (int)first[list[i]], end[i] = (int)first[list[i] + 1];
+	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += gridDim.x * blockDim.x)
+		sz[i] = i < n ? first[list[i] + 1] - first[list[i]] : 0;
 }
 
-__global__ void k_bucket_gather(const DHit *__restrict__ a, const BKey *__restrict__ key, const uint32_t *__restrict__ first, const uint32_t *list, uint32_t n,
-                                DHit *__restrict__ out)
+__global__ void k_bucket_pairs(const DHit *__restrict__ a, const uint32_t *__restrict__ first, const uint32_t *list, uint32_t n,
+                               const uint32_t *__restrict__ off, BKey *key, uint32_t *slot)
 {
 	for (uint32_t b = blockIdx.x; b < n; b += gridDim.x) {
-		const uint32_t f = first[list[b]], e = first[list[b] + 1];
-		for (uint32_t j = f + threadIdx.x; j < e; j += blockDim.x) st_hit(out + j, ld_hit(a + (uint32_t)key[j]));
+		const uint32_t f = first[list[b]], cnt = first[list[b] + 1] - f, o = off[b];
+		for (uint32_t j = threadIdx.x; j < cnt; j += blockDim.x)
+			key[o + j] = bucket_key(__ldg(reinterpret_cast<const uint2*>(a + f + j))), slot[o + j] = j;
+	}
+}
+
+__global__ void k_bucket_gather(const DHit *__restrict__ a, const uint32_t *__restrict__ first, const uint32_t *list, uint32_t n,
+                                const uint32_t *__restrict__ off, const uint32_t *__restrict__ slot, DHit *__restrict__ out)
+{
+	for (uint32_t b = blockIdx.x; b < n; b += gridDim.x) {
+		const uint32_t r = list[b], f = first[r], cnt = first[r + 1] - f, o = off[b];
+		for (uint32_t j = threadIdx.x; j < cnt; j += blockDim.x) bucket_put(out + f + j, a + f + slot[o + j], r);
 	}
 }
 
@@ -301,44 +399,48 @@ void dh_bucket_first(MabDev &d, const uint32_t *cnt, uint32_t n_seq, uint32_t *f
 	++d.n_lib;
 }
 
-void dh_sort_buckets(MabDev &d, DHits &h, const uint32_t *first, const uint64_t *key64)
+void dh_sort_buckets(MabDev &d, DHits &h, const uint32_t *first)
 {
 	drop_bounds(d, h);
 	const uint32_t n_seq = h.n_seq;
 	if (h.n == 0 || n_seq == 0) return;
-	if (h.n >= (1ull << 32)) { fprintf(stderr, "[E::miniasm_b200] more than 2^32 hits on one GPU\n"); exit(73); }
-	const BKey *key = reinterpret_cast<const BKey*>(key64);
 	h.grp = mab_alloc<uint64_t>(d, n_seq);
 	uint32_t *big = mab_alloc<uint32_t>(d, n_seq);
 	d.zero_scal(SC_BIG);
 	unsigned grid = (n_seq + BKW_WARPS - 1) / BKW_WARPS;
 	if (grid > MAB_SMS * 32u) grid = MAB_SMS * 32u;
-	MAB_LAUNCH(d, k_bucket_warp, grid, BKW_WARPS * 32, 0, h.a, key, first, n_seq, h.a2, h.grp, big, d.d_scal);
+	MAB_LAUNCH(d, k_bucket_warp, grid, BKW_WARPS * 32, 0, h.a2, first, n_seq, h.a, h.grp, big, d.d_scal);
 	const uint32_t n_big = (uint32_t)d.get_scal(SC_BIG);
 	if (n_big) {
 		const size_t smem = sizeof(typename BkcSort::TempStorage);
 		MAB_CUDA(cudaFuncSetAttribute(k_bucket_cta, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); // per device: set on every use
 		uint32_t *huge = mab_alloc<uint32_t>(d, n_big);
 		d.zero_scal(SC_AUX2);
-		MAB_LAUNCH(d, k_bucket_cta, n_big < MAB_SMS ? n_big : MAB_SMS, BKC_THREADS, smem, h.a, key, first, big, n_big, h.a2, huge, d.d_scal);
+		MAB_LAUNCH(d, k_bucket_cta, n_big < MAB_SMS ? n_big : MAB_SMS, BKC_THREADS, smem, h.a2, first, big, n_big, h.a, huge, d.d_scal);
 		const uint32_t n_huge = (uint32_t)d.get_scal(SC_AUX2);
-		if (n_huge) { // buckets beyond a CTA: a segmented sort of their keys (positions keep their bucket offsets), then the gather
-			if (h.n >= (1ull << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 hits on one GPU\n"); exit(73); }
-			BKey *sorted = mab_alloc<BKey>(d, h.n);
-			int *beg = mab_alloc<int>(d, n_huge), *end = mab_alloc<int>(d, n_huge);
-			MAB_LAUNCH(d, k_bucket_segs, mab_grid(n_huge, 128), 128, 0, huge, n_huge, first, beg, end);
+		if (n_huge) {
+			uint32_t *sz = mab_alloc<uint32_t>(d, (size_t)n_huge + 1), *off = mab_alloc<uint32_t>(d, (size_t)n_huge + 1);
+			MAB_LAUNCH(d, k_bucket_sizes, mab_grid((size_t)n_huge + 1, 128), 128, 0, huge, n_huge, first, sz);
+			dh_bucket_first(d, sz, n_huge, off);
+			uint32_t n_pair;
+			MAB_CUDA(cudaMemcpyAsync(&n_pair, off + n_huge, 4, cudaMemcpyDeviceToHost, d.stream));
+			d.sync();
+			if (n_pair >= (1u << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 hits in reads of more than %d hits on one GPU\n", BKC_HITS); exit(73); }
+			BKey *k0 = mab_alloc<BKey>(d, n_pair), *k1 = mab_alloc<BKey>(d, n_pair);
+			uint32_t *s0 = mab_alloc<uint32_t>(d, n_pair), *s1 = mab_alloc<uint32_t>(d, n_pair);
+			const unsigned g = n_huge < MAB_SMS * 4 ? n_huge : MAB_SMS * 4;
+			MAB_LAUNCH(d, k_bucket_pairs, g, 256, 0, h.a2, first, huge, n_huge, off, k0, s0);
 			size_t tb = 0;
-			cub::DeviceSegmentedSort::SortKeys(nullptr, tb, key, sorted, (int)h.n, (int)n_huge, beg, end, d.stream);
+			cub::DeviceSegmentedSort::SortPairs(nullptr, tb, k0, k1, s0, s1, (int)n_pair, (int)n_huge, off, off + 1, d.stream);
 			void *tmp = d.tmp(tb);
-			cub::DeviceSegmentedSort::SortKeys(tmp, tb, key, sorted, (int)h.n, (int)n_huge, beg, end, d.stream);
+			cub::DeviceSegmentedSort::SortPairs(tmp, tb, k0, k1, s0, s1, (int)n_pair, (int)n_huge, off, off + 1, d.stream);
 			++d.n_lib;
-			MAB_LAUNCH(d, k_bucket_gather, n_huge < MAB_SMS * 4 ? n_huge : MAB_SMS * 4, 256, 0, h.a, sorted, first, huge, n_huge, h.a2);
-			d.free(sorted); d.free(beg); d.free(end);
+			MAB_LAUNCH(d, k_bucket_gather, g, 256, 0, h.a2, first, huge, n_huge, off, s1, h.a);
+			d.free(sz); d.free(off); d.free(k0); d.free(k1); d.free(s0); d.free(s1);
 		}
 		d.free(huge);
 	}
 	d.free(big);
-	DHit *t = h.a; h.a = h.a2; h.a2 = t;
 }
 
 void dh_sort(MabDev &d, DHits &h)
@@ -348,14 +450,13 @@ void dh_sort(MabDev &d, DHits &h)
 	if (h.n == 0 || n_seq == 0) return;
 	if (h.n >= (1ull << 32)) { fprintf(stderr, "[E::miniasm_b200] more than 2^32 hits on one GPU\n"); exit(73); }
 	uint32_t *cnt = mab_alloc<uint32_t>(d, (size_t)n_seq + 1), *first = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);
-	uint64_t *key = mab_alloc<uint64_t>(d, h.n);
 	MAB_CUDA(cudaMemsetAsync(cnt, 0, ((size_t)n_seq + 1) * 4, d.stream));
 	MAB_LAUNCH(d, k_bucket_count, mab_grid(h.n, 256), 256, 0, h.a, h.n, cnt);
 	dh_bucket_first(d, cnt, n_seq, first);
 	MAB_CUDA(cudaMemsetAsync(cnt, 0, (size_t)n_seq * 4, d.stream));   // the counts become the buckets' fill cursors
-	MAB_LAUNCH(d, k_bucket_fill, mab_grid(h.n, 256), 256, 0, h.a, h.n, first, cnt, reinterpret_cast<BKey*>(key));
-	dh_sort_buckets(d, h, first, key);
-	d.free(cnt); d.free(first); d.free(key);
+	MAB_LAUNCH(d, k_bucket_fill, mab_grid(h.n, 256), 256, 0, h.a, h.n, first, cnt, h.a2);
+	dh_sort_buckets(d, h, first);
+	d.free(cnt); d.free(first);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -25,13 +25,15 @@ void dh_reserve(MabDev &d, DHits &h, size_t m);
 void dh_free(MabDev &d, DHits &h);
 
 // ma_hit_sort (hit.c:19-22): sort by the 64-bit qns (query id, then query start); stable.  A per-read bucket sort: counts per
-// query read, every hit's key (qs << 32 | input position) in its read's bucket, then each bucket sorted and its records gathered.
-// Sets h.grp.
+// query read, every record scattered into its read's bucket in h.a2 with its input position i in the query-id half of qns
+// (requires n < 2^32), then each bucket sorted by qs << 32 | i into h.a.  Sets h.grp.
 void dh_sort(MabDev &d, DHits &h);
 // The same for a caller that built the buckets itself: first = exclusive scan of the per-read counts (n_seq + 1 entries, from
-// dh_bucket_first), key[first[q] ..< first[q + 1]] = the keys of read q's hits in any order.
+// dh_bucket_first); h.a2[first[q] ..< first[q + 1]] = read q's records in any order, each with an ordinal in the query-id half of
+// qns that is distinct within the bucket and increases with the hit's input order.  Sorts every bucket by qs << 32 | ordinal into
+// the same positions of h.a, with q written back into the query-id half; h.a2 is left as scratch.
 void dh_bucket_first(MabDev &d, const uint32_t *cnt, uint32_t n_seq, uint32_t *first);
-void dh_sort_buckets(MabDev &d, DHits &h, const uint32_t *first, const uint64_t *key);
+void dh_sort_buckets(MabDev &d, DHits &h, const uint32_t *first);
 
 // ma_hit_sub (hit.c:109-160).  sub_out: n_seq entries, fully written (zeros for reads heading no group).
 // Returns the number of reads that keep an interval ("query sequences remain after sub").

@@ -15,8 +15,9 @@
 // filter and enters both names into an exact open-addressing dictionary (slot word = hash fragment + byte offset of a witness
 // occurrence: an occurrence with the same fragment compares its bytes with the witness's; value = smallest occurrence number,
 // atomicMin) -- all in ONE pass that leaves a 32-byte record per line, (3) distinct names ranked by first occurrence = ids,
-// (4) hits emitted at scanned offsets, (5) radix sort (hit_dev.cu).  ingest_paf_stream runs (1)-(2) chunk by chunk while the next
-// chunks of the text are still crossing PCIe.
+// (4) hits counted per query read, then every hit emitted straight into its read's bucket, (5) each bucket sorted
+// (dh_sort_buckets, hit_dev.cu).  ingest_paf_stream runs (1)-(2) chunk by chunk while the next chunks of the text are still
+// crossing PCIe.
 #include "ingest_dev.cuh"
 #include "shard_comm.cuh"
 #include <cub/cub.cuh>
@@ -447,36 +448,32 @@ __global__ void k_dict_rank(const unsigned long long *first_sorted, const uint64
 }
 
 // --------------------------------------------------------------------------------------------- hits
-// hits per line, and per query read (the bucket sizes of the sort, dh_sort_buckets)
-__global__ void k_hit_count(const PRec *ln, uint64_t n_lines, int bi_dir, NameTab t, uint32_t *cnt, uint32_t *read_cnt)
+// hits per query read (the bucket sizes of the sort, dh_sort_buckets)
+__global__ void k_hit_count(const PRec *ln, uint64_t n_lines, int bi_dir, NameTab t, uint32_t *read_cnt)
 {
 	for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n_lines; i += (uint64_t)gridDim.x * blockDim.x) {
 		const uint2 sl = *reinterpret_cast<const uint2*>(&ln[i].slot_q);
-		const uint32_t c = sl.x != NOSLOT ? (bi_dir && sl.x != sl.y ? 2 : 1) : 0;
-		cnt[i] = c;
-		if (c) atomicAdd(&read_cnt[t.id[sl.x]], 1u);
-		if (c == 2) atomicAdd(&read_cnt[t.id[sl.y]], 1u);
+		if (sl.x == NOSLOT) continue;
+		atomicAdd(&read_cnt[t.id[sl.x]], 1u);
+		if (bi_dir && sl.x != sl.y) atomicAdd(&read_cnt[t.id[sl.y]], 1u);
 	}
 }
 
-// hits at off[i] (file order), and every hit's sort key (qs << 32 | position) into its query read's bucket
-__global__ void k_hit_emit(const PRec *ln, uint64_t n_lines, const uint32_t *cnt, const uint64_t *off, NameTab t, DHit *out,
-                           const uint32_t *__restrict__ first, uint32_t *cur, unsigned long long *key)
+// every stored line's hit, and its mirror, straight into the bucket of its query read, with the ordinal 2 * line (+ 1 for the
+// mirror) in the query-id half of qns: the order of the ordinals is the file order of the hits, as dh_sort_buckets needs
+__global__ void k_hit_emit(const PRec *ln, uint64_t n_lines, int bi_dir, NameTab t, const uint32_t *__restrict__ first, uint32_t *cur, DHit *out)
 {
 	for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n_lines; i += (uint64_t)gridDim.x * blockDim.x) {
-		const uint32_t c = cnt[i];
-		if (c == 0) continue;
 		const PRec r = ln[i];
-		const uint32_t qid = t.id[r.slot_q], tid = t.id[r.slot_t], bl = line_bl(ln, i, 0);
-		const uint64_t p = off[i];
-		uint4 *o = reinterpret_cast<uint4*>(out + p);
-		o[0] = make_uint4(r.qs, qid, r.qe, tid);
+		if (r.slot_q == NOSLOT) continue;
+		const uint32_t qid = t.id[r.slot_q], tid = t.id[r.slot_t], bl = line_bl(ln, i, 0), ord = (uint32_t)(2 * i);
+		uint4 *o = reinterpret_cast<uint4*>(out + first[qid] + atomicAdd(&cur[qid], 1u));
+		o[0] = make_uint4(r.qs, ord, r.qe, tid);
 		o[1] = make_uint4(r.ts, r.te, r.ml_rev, bl);
-		key[first[qid] + atomicAdd(&cur[qid], 1u)] = (unsigned long long)r.qs << 32 | p;
-		if (c == 2) { // the same overlap seen from the target (hit.c:92-98)
-			o[2] = make_uint4(r.ts, tid, r.te, qid);
-			o[3] = make_uint4(r.qs, r.qe, r.ml_rev, bl);
-			key[first[tid] + atomicAdd(&cur[tid], 1u)] = (unsigned long long)r.ts << 32 | (p + 1);
+		if (bi_dir && qid != tid) { // the same overlap seen from the target (hit.c:92-98)
+			o = reinterpret_cast<uint4*>(out + first[tid] + atomicAdd(&cur[tid], 1u));
+			o[0] = make_uint4(r.ts, ord + 1, r.te, qid);
+			o[1] = make_uint4(r.qs, r.qe, r.ml_rev, bl);
 		}
 	}
 }
@@ -656,8 +653,8 @@ void ingest_paf_stream(MabDev &d, char *d_text, const char *host_text, size_t le
 static void ingest_finish(MabDev &d, const char *d_text, size_t len, uint64_t *start, PRec *ln, uint64_t n_lines, NameTab tab, uint64_t cap, int bi_dir,
                           const NoContParams *nocont, DHits &h, DNames &names, IngestStats &st)
 {
-	uint32_t *cnt = nullptr;
-	uint64_t *off = nullptr;
+	// the hit ordinals 2 * line + 1 and the bucket offsets are 32-bit
+	if (2 * n_lines >= (1ull << 32)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 PAF lines on one GPU\n"); exit(73); }
 	d.trace("ingest:dictionary");
 	if (nocont) { // -R: mark the contained reads, drop every line that names one, take the first appearances again
 		uint8_t *excl = mab_alloc<uint8_t>(d, cap);
@@ -709,41 +706,26 @@ static void ingest_finish(MabDev &d, const char *d_text, size_t len, uint64_t *s
 	d.free(slots);
 
 	d.trace("ingest:rank_ids");
-	// (5) hits at scanned offsets (file order, mirrored hit right after its original); the counts per query read and the keys in
-	// their buckets are taken on the way, so the sort starts from the buckets
-	cnt = mab_alloc<uint32_t>(d, n_lines);
-	off = mab_alloc<uint64_t>(d, n_lines + 1);
+	// (5) hits counted per query read, then emitted straight into their read's bucket of h.a2
 	uint32_t *read_cnt = mab_alloc<uint32_t>(d, (size_t)n_seq + 1), *first = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);
 	MAB_CUDA(cudaMemsetAsync(read_cnt, 0, ((size_t)n_seq + 1) * 4, d.stream));
-	MAB_LAUNCH(d, k_hit_count, mab_grid(n_lines, 256), 256, 0, ln, n_lines, bi_dir, tab, cnt, read_cnt);
+	MAB_LAUNCH(d, k_hit_count, mab_grid(n_lines, 256), 256, 0, ln, n_lines, bi_dir, tab, read_cnt);
 	dh_bucket_first(d, read_cnt, n_seq, first);
 	MAB_CUDA(cudaMemsetAsync(read_cnt, 0, (size_t)n_seq * 4, d.stream)); // the counts become the buckets' fill cursors
-	{
-		size_t tb = 0;
-		cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt, off, (int64_t)n_lines, d.stream);
-		void *tmp = d.tmp(tb);
-		cub::DeviceScan::ExclusiveSum(tmp, tb, cnt, off, (int64_t)n_lines, d.stream);
-		++d.n_lib;
-	}
-	uint64_t last_off;
-	uint32_t last_cnt;
-	MAB_CUDA(cudaMemcpyAsync(&last_off, off + n_lines - 1, 8, cudaMemcpyDeviceToHost, d.stream));
-	MAB_CUDA(cudaMemcpyAsync(&last_cnt, cnt + n_lines - 1, 4, cudaMemcpyDeviceToHost, d.stream));
+	uint32_t n_hits;
+	MAB_CUDA(cudaMemcpyAsync(&n_hits, first + n_seq, 4, cudaMemcpyDeviceToHost, d.stream));
 	d.sync();
-	const uint64_t n_hits = last_off + last_cnt;
-	if (n_hits >= (1ull << 32)) { fprintf(stderr, "[E::miniasm_b200] more than 2^32 hits on one GPU\n"); exit(73); }
 	dh_reserve(d, h, n_hits ? n_hits : 1);
 	h.n = n_hits, h.n_seq = n_seq;
-	uint64_t *key = mab_alloc<uint64_t>(d, n_hits);
-	if (n_hits) MAB_LAUNCH(d, k_hit_emit, mab_grid(n_lines, 256), 256, 0, ln, n_lines, cnt, off, tab, h.a, first, read_cnt, (unsigned long long*)key);
+	if (n_hits) MAB_LAUNCH(d, k_hit_emit, mab_grid(n_lines, 256), 256, 0, ln, n_lines, bi_dir, tab, first, read_cnt, h.a2);
 	st.n_hits = n_hits, st.n_seq = n_seq;
-	d.free(cnt); d.free(off); d.free(ln); d.free(start);
+	d.free(ln); d.free(start);
 	d.free(tab.key); d.free(tab.first); d.free(tab.id);
 
 	d.trace("ingest:emit_hits");
-	// (6) ma_hit_sort: order every bucket
-	dh_sort_buckets(d, h, first, key);
-	d.free(read_cnt); d.free(first); d.free(key);
+	// (6) ma_hit_sort: order every bucket (h.a2 -> h.a)
+	dh_sort_buckets(d, h, first);
+	d.free(read_cnt); d.free(first);
 	d.trace("ingest:sort_hits");
 }
 
