@@ -188,6 +188,12 @@ float mab_coverage(const mab_ctx_t *ctx);
  * unitig sequences, formatted on the GPU and written with one fwrite: no host copies of the tables.  Returns the number
  * of bytes written, -1 before mab_unitigs.  (The CLI's default writer; MAB_GPU_GFA=0 selects the host route.) */
 long mab_write_gfa(mab_ctx_t *ctx, FILE *fp);
+/* The other outputs of the reference's -p, formatted on the GPU and written in chunks of bounded size (device scratch and pinned
+ * memory do not grow with the output).  Each returns the number of bytes written and exits with code 74 on a short write.
+ * They work on a single-GPU context and on rank 0's context after mab_layout_sharded. */
+long mab_write_paf(mab_ctx_t *ctx, FILE *fp); /* print_hits of main.c:21-30; -1 (nothing written) when no read selection ran */
+long mab_write_bed(mab_ctx_t *ctx, FILE *fp); /* print_subs of main.c:13-19; -1 when no read selection ran */
+long mab_write_sg(mab_ctx_t *ctx, FILE *fp);  /* ma_sg_print(mab_export_sg, mab_export_dict, mab_export_sub); -1 before mab_layout */
 /* -f reads: ma_ug_seq (asm.c:236-290) + ma_ug_print on the GPU.  mab_reads_prefetch starts streaming the FASTA/FASTQ file (plain
  * or gzip, "-" = stdin) into HBM on a thread and stream of its own -- call it before mab_ingest and the copy hides behind the
  * graph stages.  mab_write_gfa_reads indexes the records in HBM (line starts, headers, a name table of the layout's reads),

@@ -152,6 +152,9 @@ _PRODUCT_ONLY = {
     "mab_export_ug": (C.POINTER(MaUg), [C.c_void_p]),
     "mab_coverage": (C.c_float, [C.c_void_p]),
     "mab_write_gfa": (C.c_long, [C.c_void_p, C.c_void_p]),
+    "mab_write_paf": (C.c_long, [C.c_void_p, C.c_void_p]),
+    "mab_write_bed": (C.c_long, [C.c_void_p, C.c_void_p]),
+    "mab_write_sg": (C.c_long, [C.c_void_p, C.c_void_p]),
     "mab_reads_prefetch": (C.c_int, [C.c_void_p, C.c_char_p]),
     "mab_write_gfa_reads": (C.c_long, [C.c_void_p, C.c_void_p, C.c_char_p]),
     "mab_event_create": (C.c_void_p, []),

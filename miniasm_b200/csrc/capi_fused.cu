@@ -6,6 +6,7 @@
 #include "hit_dev.cuh"
 #include "clean_dev.cuh"
 #include "gfa_dev.cuh"
+#include "dump_dev.cuh"
 #include "ugseq_dev.cuh"
 #include <pthread.h>
 #include "ingest_dev.cuh"
@@ -36,7 +37,7 @@ struct mab_ctx {
 	bool have_sg = false, have_ug = false;
 	float cov = 40.0f;
 	mab_stats_t stats;
-	// pinned staging for file loads
+	// pinned staging for file loads, and the landing buffers of mab_write_paf / _bed / _sg
 	char *pin[2] = {nullptr, nullptr};
 	size_t pin_bytes = 0;
 	// sharded runs (mab_shard_init): communicator + the packed names of all ranks (names.off indexes it instead of d_text)
@@ -587,6 +588,38 @@ long mab_write_gfa(mab_ctx_t *c, FILE *fp)
 	d.free(d_txt);
 	d.sync();
 	return (long)n;
+}
+
+/* -p paf | bed | sg: the text formatted on the GPU (dump_dev.cu) and written in chunks; names come from the context's name table
+ * (name_text after a sharded ingest), intervals from its table of the current reads */
+static long write_dump(mab_ctx *c, DumpKind kind, uint64_t n_rec, FILE *fp)
+{
+	const DumpView v{{c->orig_id, c->names.off, c->names.nlen, c->name_text ? c->name_text : c->d_text, c->sub}, c->hits.a, c->sg.arc};
+	return (long)dg_dump_write(c->dev, kind, v, n_rec, fp, c->pin, c->pin_bytes);
+}
+
+/* print_hits (main.c:21-30) of the current hits; -1 (nothing written) when no read selection ran */
+long mab_write_paf(mab_ctx_t *c, FILE *fp)
+{
+	MAB_CUDA(cudaSetDevice(c->dev.device));
+	if (!c->sub) return -1;
+	return write_dump(c, DUMP_PAF, c->hits.n, fp);
+}
+
+/* print_subs (main.c:13-19) of the current reads; -1 (nothing written) when no read selection ran */
+long mab_write_bed(mab_ctx_t *c, FILE *fp)
+{
+	MAB_CUDA(cudaSetDevice(c->dev.device));
+	if (!c->sub) return -1;
+	return write_dump(c, DUMP_BED, c->n_seq, fp);
+}
+
+/* ma_sg_print (asm.c:41-55) of the string graph; -1 before mab_layout */
+long mab_write_sg(mab_ctx_t *c, FILE *fp)
+{
+	MAB_CUDA(cudaSetDevice(c->dev.device));
+	if (!c->have_sg) return -1;
+	return write_dump(c, DUMP_SG, c->sg.n_arc, fp);
 }
 
 /* ---- -f reads (ma_ug_seq, asm.c:236-290) ------------------------------------------------------------------------------- */

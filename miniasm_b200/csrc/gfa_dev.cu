@@ -15,61 +15,24 @@
 // carries "*"; with them (-f reads) it reserves `len` bytes, pre-filled with 'N', that ugseq_dev.cu fills in place.
 // This is the default writer of the CLI and of bench.py (MAB_GPU_GFA=0 / --host-gfa: host structs + ma_ug_print).
 #include "gfa_dev.cuh"
+#include "fmt_sink.cuh"
 #include <cub/cub.cuh>
 
 struct GfaView {
 	const DUtgMeta *meta; const uint64_t *items; const uint32_t *ioff; // ioff: exclusive (mod 2^32) sum of item lengths
 	uint32_t n_utg; uint64_t n_items;
 	const DArc *uarc; uint32_t n_uarc; const uint64_t *uidx;
-	const uint32_t *orig; const uint64_t *noff; const uint32_t *nlen; const char *text; const DSub *sub;
+	ReadNames nm;
 	uint64_t *seq_pos;             // non-null: S lines reserve `len` bytes for the unitig sequence; seq_pos[i] = where (filled by the write pass)
 	const char *out_base;
 };
 
-struct CountSink {
-	uint32_t n;
-	__host__ __device__ __forceinline__ void c(char) { ++n; }
-	__host__ __device__ __forceinline__ void bytes(const char *, uint32_t l) { n += l; }
-	__host__ __device__ __forceinline__ void hole(uint32_t l, uint64_t *, const char *) { n += l; }
-};
-struct WriteSink {
-	char *p;
-	__host__ __device__ __forceinline__ void c(char ch) { *p++ = ch; }
-	__host__ __device__ __forceinline__ void bytes(const char *s, uint32_t l) { for (uint32_t k = 0; k < l; ++k) p[k] = s[k]; p += l; }
-	__host__ __device__ __forceinline__ void hole(uint32_t l, uint64_t *where, const char *base) { *where = (uint64_t)(p - base); p += l; } // left as the buffer was pre-filled
-};
-
-template <class Sink> __host__ __device__ __forceinline__ void put_dec(Sink &s, uint32_t x, int min_digits)
-{
-	char t[10];
-	int n = 0;
-	do t[n++] = (char)('0' + x % 10), x /= 10; while (x);
-	for (int k = n; k < min_digits; ++k) s.c('0');
-	while (n) s.c(t[--n]);
-}
-template <class Sink> __host__ __device__ __forceinline__ void put_int(Sink &s, int32_t v) // "%d"
-{
-	uint32_t x = (uint32_t)v;
-	if (v < 0) s.c('-'), x = 0u - x;
-	put_dec(s, x, 1);
-}
 template <class Sink> __host__ __device__ __forceinline__ void put_utg(Sink &s, uint32_t i, bool circ) // "utg%.6d%c" of i + 1
 {
 	s.c('u'); s.c('t'); s.c('g');
 	put_dec(s, i + 1, 6);
 	s.c(circ ? 'c' : 'l');
 }
-template <class Sink> __host__ __device__ __forceinline__ void put_read(Sink &s, const GfaView &v, uint32_t r) // name or name:s+1-e
-{
-	const uint32_t o = v.orig ? v.orig[r] : r;
-	s.bytes(v.text + v.noff[o], v.nlen[o]);
-	if (v.sub) {
-		const DSub b = v.sub[r];
-		s.c(':'); put_int(s, (int32_t)((b.s_del & 0x7fffffffu) + 1)); s.c('-'); put_int(s, (int32_t)b.e);
-	}
-}
-template <class Sink> __host__ __device__ __forceinline__ void put_lit(Sink &s, const char *lit, uint32_t l) { for (uint32_t k = 0; k < l; ++k) s.c(lit[k]); }
-
 template <class Sink> __host__ __device__ void emit_record(const GfaView &v, uint64_t rec, Sink &s)
 {
 	const uint64_t n_block = (uint64_t)v.n_utg + v.n_items;
@@ -97,7 +60,7 @@ template <class Sink> __host__ __device__ void emit_record(const GfaView &v, uin
 			const uint64_t it = v.items[k];
 			const uint32_t off = v.ioff[k] - v.ioff[m.first];
 			s.c('a'); s.c('\t'); put_utg(s, i, m.circ != 0); s.c('\t'); put_int(s, (int32_t)off); s.c('\t');
-			put_read(s, v, (uint32_t)(it >> 33));
+			put_read(s, v.nm, (uint32_t)(it >> 33));
 			s.c('\t'); s.c((it >> 32 & 1) ? '-' : '+'); s.c('\t'); put_int(s, (int32_t)(uint32_t)it); s.c('\n');
 		}
 	} else if (rec < n_block + v.n_uarc) {
@@ -115,8 +78,8 @@ template <class Sink> __host__ __device__ void emit_record(const GfaView &v, uin
 		} else {
 			put_utg(s, i, false); s.c('\t'); put_int(s, (int32_t)m.len); s.c('\t'); put_int(s, (int32_t)m.n); s.c('\t');
 			put_int(s, (int32_t)(uint32_t)v.uidx[(size_t)i << 1 | 1]); s.c('\t'); put_int(s, (int32_t)(uint32_t)v.uidx[(size_t)i << 1 | 0]); s.c('\t');
-			put_read(s, v, m.start >> 1); s.c('\t'); s.c((m.start & 1) ? '-' : '+'); s.c('\t');
-			put_read(s, v, m.end >> 1); s.c('\t'); s.c((m.end & 1) ? '-' : '+'); s.c('\n');
+			put_read(s, v.nm, m.start >> 1); s.c('\t'); s.c((m.start & 1) ? '-' : '+'); s.c('\t');
+			put_read(s, v.nm, m.end >> 1); s.c('\t'); s.c((m.end & 1) ? '-' : '+'); s.c('\n');
 		}
 	}
 }
@@ -161,7 +124,7 @@ size_t dg_gfa_text(MabDev &d, const DUnitigs &ug, const uint32_t *orig, const ui
 		cub::DeviceScan::ExclusiveSum(tmp, tb, in, ioff, (int64_t)ug.n_items, d.stream);
 		++d.n_lib;
 	}
-	GfaView v{ug.meta, ug.items, ioff, ug.n_utg, ug.n_items, ug.g.arc, ug.g.n_arc, ug.g.idx, orig, noff, nlen, name_text, sub, seq_pos, nullptr};
+	GfaView v{ug.meta, ug.items, ioff, ug.n_utg, ug.n_items, ug.g.arc, ug.g.n_arc, ug.g.idx, {orig, noff, nlen, name_text, sub}, seq_pos, nullptr};
 	uint32_t *len = mab_alloc<uint32_t>(d, n_rec);
 	uint64_t *pos = mab_alloc<uint64_t>(d, n_rec + 1);
 	MAB_LAUNCH(d, k_gfa_count, mab_grid(n_rec, 256), 256, 0, v, n_rec, len);
@@ -207,7 +170,7 @@ extern "C" size_t mab_test_gfa_host(const ma_ug_t *ug, const sdict_t *d, const m
 	std::vector<uint32_t> nlen(d->n_seq ? d->n_seq : 1);
 	for (uint32_t r = 0; r < d->n_seq; ++r) noff[r] = text.size(), nlen[r] = (uint32_t)strlen(d->seq[r].name), text += d->seq[r].name;
 	GfaView v{meta.data(), items.data(), ioff.data(), (uint32_t)ug->u.n, (uint64_t)items.size(),
-	          (const DArc*)ug->g->arc, ug->g->n_arc, ug->g->idx, nullptr, noff.data(), nlen.data(), text.data(), (const DSub*)sub, nullptr, nullptr};
+	          (const DArc*)ug->g->arc, ug->g->n_arc, ug->g->idx, {nullptr, noff.data(), nlen.data(), text.data(), (const DSub*)sub}, nullptr, nullptr};
 	const uint64_t n_rec = (uint64_t)v.n_utg * 2 + v.n_items + v.n_uarc;
 	size_t tot = 0;
 	for (uint64_t r = 0; r < n_rec; ++r) { CountSink s{0}; emit_record(v, r, s); tot += s.n; }

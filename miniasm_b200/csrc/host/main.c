@@ -17,24 +17,6 @@
 
 #define MAB_VERSION "0.3-r179"   /* tracks the reference release whose output it reproduces */
 
-static void write_bed(const sdict_t *d, const ma_sub_t *sub) /* -p bed, main.c:13-19 */
-{
-	uint32_t i;
-	for (i = 0; i < d->n_seq; ++i)
-		if (!d->seq[i].del && sub[i].s != sub[i].e)
-			printf("%s\t%d\t%d\n", d->seq[i].name, sub[i].s, sub[i].e);
-}
-
-static void write_paf(size_t n, const ma_hit_t *h, const sdict_t *d, const ma_sub_t *sub) /* -p paf, main.c:21-30 */
-{
-	size_t i;
-	for (i = 0; i < n; ++i) {
-		uint32_t q = (uint32_t)(h[i].qns >> 32), t = h[i].tn;
-		printf("%s:%d-%d\t%d\t%d\t%d\t%c\t%s:%d-%d\t%d\t%d\t%d\t%d\t%d\t255\n", d->seq[q].name, sub[q].s + 1, sub[q].e, sub[q].e - sub[q].s,
-			   (uint32_t)h[i].qns, h[i].qe, "+-"[h[i].rev], d->seq[t].name, sub[t].s + 1, sub[t].e, sub[t].e - sub[t].s, h[i].ts, h[i].te, h[i].ml, h[i].bl);
-	}
-}
-
 static void usage(const ma_opt_t *o, const char *outfmt)
 {
 	fprintf(stderr, "Usage: miniasm-b200 [options] <in.paf>\n");
@@ -246,14 +228,9 @@ int main(int argc, char *argv[])
 	if (!sharded_done) mab_select(ctx, &opt, no_first, no_second, stage); /* prints the Step 2 / Step 3 banners where the reference does */
 
 	if (strcmp(outfmt, "bed") == 0) {
-		d = mab_export_dict(ctx), sub = mab_export_sub(ctx);
-		if (sub) write_bed(d, sub);
+		mab_write_bed(ctx, out);     /* print_subs, formatted on the GPU; nothing when no read selection ran (-1 -2) */
 	} else if (strcmp(outfmt, "paf") == 0) {
-		size_t n_hits;
-		ma_hit_t *hit = mab_export_hits(ctx, &n_hits);
-		d = mab_export_dict(ctx), sub = mab_export_sub(ctx);
-		if (sub) write_paf(n_hits, hit, d, sub);
-		free(hit);
+		mab_write_paf(ctx, out);     /* print_hits, likewise */
 	} else if (strcmp(outfmt, "ug") == 0 || strcmp(outfmt, "sg") == 0) {
 		/* no -f: the GFA text is formatted on the GPU and copied down once (MAB_GPU_GFA=0: host structs + ma_ug_print) */
 		const int gpu_gfa = strcmp(outfmt, "ug") == 0 && !fn_reads && !((env = getenv("MAB_GPU_GFA")) != 0 && atoi(env) == 0);
@@ -277,10 +254,7 @@ int main(int argc, char *argv[])
 				ma_ug_destroy(ug);
 			}
 		} else {
-			asg_t *sg = mab_export_sg(ctx);
-			d = mab_export_dict(ctx), sub = mab_export_sub(ctx);
-			ma_sg_print(sg, d, sub, out);
-			asg_destroy(sg);
+			mab_write_sg(ctx, out);      /* ma_sg_print, formatted on the GPU */
 		}
 	}
 	if (out != stdout) fclose(out);
