@@ -8,6 +8,7 @@
 #include "clean_dev.cuh"
 #include "clean_fix.cuh"
 #include <cub/cub.cuh>
+#include <algorithm>
 
 thread_local CleanStats g_clean_stats;
 static inline void clean_note(uint32_t rounds, uint32_t committed)
@@ -188,9 +189,9 @@ __global__ void k_fx_bub_sweep(FxView g, uint32_t max_dist, FxSlots sl, const ui
 	}
 }
 
-static void fx_slots_alloc(MabDev &d, FxSlots &sl, uint32_t n_slot, uint32_t bcap)
+static void fx_slots_alloc(MabDev &d, FxSlots &sl, uint32_t n_slot, uint32_t bcap, uint32_t ecap)
 {
-	sl.n_slot = n_slot, sl.bcap = bcap, sl.ecap = bcap * 4;
+	sl.n_slot = n_slot, sl.bcap = bcap, sl.ecap = ecap;
 	sl.hcap = 1; while (sl.hcap < 2 * bcap) sl.hcap <<= 1;
 	const size_t nh = (size_t)n_slot * sl.hcap, nb = (size_t)n_slot * sl.bcap, ne = (size_t)n_slot * sl.ecap;
 	sl.hkey = mab_alloc<uint32_t>(d, nh); sl.hp = mab_alloc<uint32_t>(d, nh); sl.hd = mab_alloc<uint32_t>(d, nh);
@@ -221,17 +222,21 @@ uint64_t dg_pop_bubble(MabDev &d, DGraph &g, int max_dist)
 			FxBuf b;
 			fx_alloc(d, g, b);
 			FxSlots sl;
-			uint32_t bcap = 64, n_slot = n_src < 16384 ? (n_src + 63) / 64 * 64 : 16384;
-			fx_slots_alloc(d, sl, n_slot, bcap);
+			uint32_t bcap = 64, ecap = 256, n_slot = n_src < 16384 ? (n_src + 63) / 64 * 64 : 16384;
+			fx_slots_alloc(d, sl, n_slot, bcap, ecap);
 			for (;;) {
 				d.zero_scal(SC_TMP0, 4);
 				MAB_LAUNCH(d, k_fx_bub_sweep, (sl.n_slot + 63) / 64, 64, 0, fx_view(g, b), (uint32_t)max_dist, sl, src, n_src, d.d_scal + SC_TMP0);
 				if (d.get_scal(SC_TMP0 + 2)) { // a traversal outgrew its scratch slot: enlarge, re-arm T_new and redo the sweep
+					// A walk visits each vertex other than its source at most once and scans each arc at most once, so with
+					// bcap >= n_vtx and ecap >= n_arc no walk can overflow; the arc list grows with the arcs a walk scans,
+					// which a dense graph makes far more than 4 per vertex, so each capacity grows up to its own bound.
+					if (bcap >= n_vtx && ecap >= g.n_arc) { fprintf(stderr, "[E::miniasm_b200] bubble scratch overflow\n"); exit(75); }
 					fx_slots_free(d, sl);
-					bcap *= 4;
+					bcap = (uint32_t)std::min<uint64_t>((uint64_t)bcap * 4, std::max(bcap, n_vtx));
+					ecap = (uint32_t)std::min<uint64_t>((uint64_t)ecap * 4, std::max(ecap, g.n_arc));
 					if (n_slot > 64) n_slot /= 4;
-					if ((uint64_t)bcap > (uint64_t)n_vtx * 4) { fprintf(stderr, "[E::miniasm_b200] bubble scratch overflow\n"); exit(75); }
-					fx_slots_alloc(d, sl, n_slot, bcap);
+					fx_slots_alloc(d, sl, n_slot, bcap, ecap);
 					MAB_LAUNCH(d, k_fx_init, mab_grid((size_t)g.n_arc + g.n_seq, 256), 256, 0, g.arc, g.seq, g.n_arc, g.n_seq,
 					           b.ts[b.cur ^ 1], b.ts[b.cur ^ 1], b.ta[b.cur ^ 1], b.ta[b.cur ^ 1]);
 					continue;
