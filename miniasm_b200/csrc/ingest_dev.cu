@@ -11,13 +11,13 @@
 //   * every stored line yields a hit and, when bi_dir and query != target, the mirrored hit right after it;
 //   * hits sorted by (query id, query start).
 //
-// GPU shape: (1) line starts (newline count per tile, scan, positions), (2) one thread per line parses it, applies the store
-// filter and enters both names into an exact open-addressing dictionary (slot word = hash fragment + byte offset of a witness
-// occurrence: an occurrence with the same fragment compares its bytes with the witness's; value = smallest occurrence number,
-// atomicMin) -- all in ONE pass that leaves a 32-byte record per line, (3) distinct names ranked by first occurrence = ids,
-// (4) hits counted per query read, then every hit emitted straight into its read's bucket, (5) each bucket sorted
-// (dh_sort_buckets, hit_dev.cu).  ingest_paf_stream runs (1)-(2) chunk by chunk while the next chunks of the text are still
-// crossing PCIe.
+// GPU shape: (1) line starts (per 8 KB tile, numbered by a decoupled look-back over the tiles) and (2) one thread per line parses
+// it, applies the store filter, enters both names into an exact open-addressing dictionary (slot word = hash fragment + byte offset
+// of a witness occurrence: an occurrence with the same fragment compares its bytes with the witness's; value = smallest occurrence
+// number, atomicMin) and counts the line's hits per slot -- all in ONE pass over the text that leaves a 32-byte record per line,
+// (3) distinct names ranked by first occurrence = ids, the slot counts become per-read counts, (4) every hit emitted straight into
+// its read's bucket, (5) each bucket sorted (dh_sort_buckets, hit_dev.cu).  ingest_paf_stream runs (1)-(2) chunk by chunk while
+// the next chunks of the text are still crossing PCIe.
 #include "ingest_dev.cuh"
 #include "shard_comm.cuh"
 #include <cub/cub.cuh>
@@ -40,6 +40,7 @@ static_assert(sizeof(PRec) == 32, "PRec layout");
 constexpr uint32_t NOSLOT = 0xffffffffu;
 
 // ---- line starts -----------------------------------------------------------------------------------------
+// (dev_line_starts, for the reads file of -f in ugseq_dev.cu; the PAF parse finds its own lines, k_parse_tiles below.)
 // A line starts at byte 0 and after every '\n' that is not the last byte.  Tiles of NL_TILE bytes, one CTA each,
 // 128-bit loads laid out so that a warp reads 512 contiguous bytes per instruction.
 constexpr int NL_THREADS = 256;
@@ -95,58 +96,6 @@ __global__ void __launch_bounds__(NL_THREADS) k_nl_write(const char *__restrict_
 			__syncthreads();
 		}
 	}
-}
-
-// Streaming variants (ingest_paf_stream): tiles [t0, t1) of the text have just arrived.  nl_state[0] = newline-started lines
-// seen so far (line 0 starts at byte 0 and is not counted), nl_state[1] = capacity of `out`.
-__global__ void __launch_bounds__(NL_THREADS) k_nl_count_range(const char *__restrict__ text, size_t len, uint64_t t0, uint64_t t1, uint64_t *cnt)
-{
-	typedef cub::BlockReduce<uint32_t, NL_THREADS> BR;
-	__shared__ typename BR::TempStorage ts;
-	for (uint64_t t = t0 + blockIdx.x; t < t1; t += gridDim.x) {
-		uint32_t c = 0;
-		#pragma unroll
-		for (int k = 0; k < NL_PER_THREAD; ++k) c += __popc(nl_bits16(text, len, t * NL_TILE + ((uint64_t)k * NL_THREADS + threadIdx.x) * 16));
-		c = BR(ts).Sum(c);
-		if (threadIdx.x == 0) cnt[t - t0] = c;
-		__syncthreads();
-	}
-}
-
-__global__ void __launch_bounds__(NL_THREADS) k_nl_write_range(const char *__restrict__ text, size_t len, uint64_t t0, uint64_t t1, const uint64_t *__restrict__ base,
-                                                              const unsigned long long *nl_state, uint64_t *out)
-{
-	typedef cub::BlockScan<uint32_t, NL_THREADS> BS;
-	__shared__ typename BS::TempStorage ts;
-	const uint64_t seen = nl_state[0], cap = nl_state[1];
-	for (uint64_t t = t0 + blockIdx.x; t < t1; t += gridDim.x) {
-		uint64_t at = seen + base[t - t0];
-		#pragma unroll
-		for (int k = 0; k < NL_PER_THREAD; ++k) {
-			const uint64_t off = t * NL_TILE + ((uint64_t)k * NL_THREADS + threadIdx.x) * 16;
-			uint32_t bits = nl_bits16(text, len, off), rank, total;
-			BS(ts).ExclusiveSum((uint32_t)__popc(bits), rank, total);
-			uint64_t q = at + rank;
-			while (bits) { const int b = __ffs(bits) - 1; if (q + 1 < cap) out[q + 1] = off + b + 1; ++q; bits &= bits - 1; }
-			at += total;
-			__syncthreads();
-		}
-	}
-}
-
-// after the tiles [t0, t1): lines whose END is known now are [rng[0], rng[1]); rng[2] = total number of lines once the text is complete
-__global__ void k_nl_advance(unsigned long long *nl_state, const uint64_t *base, const uint64_t *cnt, uint64_t n_tiles, unsigned long long *rng, int last)
-{
-	if (blockIdx.x || threadIdx.x) return;
-	const unsigned long long seen = nl_state[0] + (n_tiles ? base[n_tiles - 1] + cnt[n_tiles - 1] : 0);
-	nl_state[0] = seen;
-	const unsigned long long known_starts = seen + 1;                 // lines 0 .. seen have a start
-	unsigned long long cap = nl_state[1];
-	unsigned long long hi = last ? known_starts : known_starts - 1;   // the last known line's end is the next line's start, or the end of the text
-	if (hi > cap - 1) hi = cap - 1;                                   // (overflow of the estimate: start[] is only filled below cap; the host notices and falls back)
-	rng[0] = rng[1] > hi ? hi : rng[1];                               // previous upper bound becomes the lower one
-	rng[1] = hi;
-	rng[2] = last ? known_starts : ~0ull;
 }
 
 // strtol(field, 0, 10) narrowed to uint32, on the byte range [p, e).  Up to 18 significant digits cannot
@@ -260,6 +209,7 @@ struct NameTab {
 	unsigned long long *first;
 	uint32_t *id;                // read id of the slot (after ranking)
 	uint64_t mask;
+	uint32_t *hits = nullptr;    // optional: hits whose query read is the slot's name (the bucket sizes of the hit sort)
 };
 constexpr int NT_OFF_BITS = 37;
 constexpr unsigned long long NT_OFF_MASK = (1ull << NT_OFF_BITS) - 1;
@@ -293,65 +243,162 @@ __device__ __forceinline__ uint32_t tab_insert(const NameTab &t, const char *__r
 	return 0;
 }
 
-// One CTA parses PARSE_LINES consecutive lines.  Their bytes are contiguous in the file, so the CTA first copies
-// the whole range into shared memory with coalesced 128-bit loads and the threads then walk their own line there:
-// byte-wise walking of global memory makes every warp-level load touch ~16 cache lines (L1 wavefront bound).
-// A range that does not fit (very long lines) is parsed straight from global memory.
-// Fused into the same pass (round 1 ran them as three more sweeps over a 64-byte record): the store filter of
-// hit.c:85 and the dictionary insert of both names, while the line is still in shared memory.
-constexpr int PARSE_LINES = 128;
-constexpr int PARSE_SMEM = 16 * 1024;
+// ---- the parse: one pass over the text finds the lines, numbers them, parses them and enters their names ------------
+// The text is cut into tiles of PT_TILE bytes.  Line 0 belongs to tile 0 and every other line to the tile that holds the
+// '\n' ending the line before it.  A CTA takes the next tile from a counter, so tiles start in index order and the
+// look-back below only ever waits on tiles that are already running.  The CTA
+//   * stages its tile and PT_OVER bytes after it in shared memory with 128-bit loads (byte-wise walking of global
+//     memory makes every warp-level load touch ~16 cache lines),
+//   * counts the line starts of the tile there and publishes the count; a single-pass decoupled look-back over the
+//     tiles (cub::TilePrefixCallbackOp) returns the global number of its first line,
+//   * lists the starts and hands one line to each thread, which parses it, applies the store filter of hit.c:85 and
+//     enters both names into the dictionary while the line is still in shared memory, then writes start[line] and the
+//     32-byte record, and (optionally) adds the line's hits to the bucket sizes of its slots.
+// The tile's last line is the only one that can end past the staged bytes: it is parsed straight from global memory.
+// Lines numbered line_cap or more are counted but not parsed (the host parses again with room for all of them).
+constexpr int PT_THREADS = 128;
+constexpr uint32_t PT_TILE = 8192;
+constexpr uint32_t PT_OVER = 1024;
+constexpr uint32_t PT_LIST = 1024;                       // line starts listed at once: a tile with more lines is parsed in rounds
+static_assert(PT_TILE == PT_THREADS * 64, "each thread scans 64 bytes of its tile for line starts");
+static_assert(PT_OVER % 16 == 0 && PT_OVER <= PT_TILE, "the overhang ends inside the tile after the parsed ones");
 
-__global__ void __launch_bounds__(PARSE_LINES)
-k_parse(const char *__restrict__ text, size_t len, const uint64_t *__restrict__ start, const unsigned long long *__restrict__ rng,
-        int min_span, int min_match, NameTab tab, PRec *out, unsigned long long *counts)
-{	// rng: lines [rng[0], rng[1]) are parsed; rng[2] = number of lines of the whole text, or ~0 while it is still arriving (then
-	// line rng[1] exists and its start ends line rng[1]-1).  counts: [0] lines with >= 10 fields, [1] lines stored, [2] dictionary overflow
-	__shared__ __align__(16) char s_text[PARSE_SMEM];
-	__shared__ uint32_t s_vals[PARSE_LINES / 32][11][32];
-	unsigned n_parsed = 0, n_pass = 0;
-	const uint64_t line_lo = rng[0], line_hi = rng[1], n_lines = rng[2];
-	const uint64_t n_blk = (line_hi - line_lo + PARSE_LINES - 1) / PARSE_LINES;
-	for (uint64_t b = blockIdx.x; b < n_blk; b += gridDim.x) {
-		const uint64_t l0 = line_lo + b * PARSE_LINES, l1 = l0 + PARSE_LINES < line_hi ? l0 + PARSE_LINES : line_hi;
-		const uint64_t s0 = start[l0], s1 = l1 < n_lines ? start[l1] : len;
-		const uint64_t a0 = s0 & ~(uint64_t)15;
-		const bool staged = s1 - a0 <= PARSE_SMEM;
-		__syncthreads(); // the previous range is no longer needed
-		if (staged) {
-			const uint64_t n16 = (s1 - a0 + 15) >> 4; // whole 16-byte words; the tail word may reach past `len` but stays inside the (padded) allocation
-			for (uint64_t k = threadIdx.x; k < n16; k += PARSE_LINES)
-				reinterpret_cast<uint4*>(s_text)[k] = __ldg(reinterpret_cast<const uint4*>(text + a0) + k);
-		}
-		__syncthreads();
-		const uint64_t i = l0 + threadIdx.x;
-		if (i < l1) {
-			const uint64_t s = start[i];
-			uint64_t eol = i + 1 < n_lines ? start[i + 1] - 1 : (text[len - 1] == '\n' ? len - 1 : len);
-			const char *base = staged ? s_text - a0 : text; // base + file offset = address of that byte
-			if (eol - s > 1 && base[eol - 1] == '\r') --eol;
-			PLine r;
-			parse_line(base + s, base + eol, r, &s_vals[threadIdx.x >> 5][0][threadIdx.x & 31]);
-			PRec o;
-			o.qs = r.qs, o.qe = r.qe, o.ts = r.ts, o.te = r.te, o.ml_rev = r.ml_rev;
-			o.bl_f = (r.bl & 0x7fffffffu) | (r.nf >= 11 ? 0x80000000u : 0u);
-			o.slot_q = NOSLOT, o.slot_t = 0;
-			if (r.nf >= 10) {
-				++n_parsed;
-				if (!(r.qe - r.qs < (uint32_t)min_span || r.te - r.ts < (uint32_t)min_span || (int)(r.ml_rev & 0x7fffffffu) < min_match)) {
-					++n_pass;
-					o.slot_q = tab_insert(tab, text, base + s, r.qnl, s, 2 * i, counts + 2);
-					o.slot_t = tab_insert(tab, text, base + s + r.tdelta, r.tnl, s + r.tdelta, 2 * i + 1, counts + 2);
-				}
-			}
-			*reinterpret_cast<uint4*>(out + i) = make_uint4(o.qs, o.qe, o.ts, o.te);
-			*(reinterpret_cast<uint4*>(out + i) + 1) = make_uint4(o.ml_rev, o.bl_f, o.slot_q, o.slot_t);
+typedef cub::ScanTileState<unsigned long long> LineTileState;
+typedef cub::TilePrefixCallbackOp<unsigned long long, ::cuda::std::plus<unsigned long long>, LineTileState> LinePrefixOp;
+
+// counts[]: [0] lines with >= 10 fields, [1] lines stored, [2] dictionary overflow, [3] lines of the text (set by its last tile),
+// [4] lines that run past the bytes that have arrived
+enum { PC_PARSED = 0, PC_STORED, PC_OVERFLOW, PC_LINES, PC_CUT, PC_N };
+
+__device__ __forceinline__ uint32_t nl_bits_u4(const uint4 w)  // bit k = byte k of the 16 bytes is '\n'
+{
+	const uint32_t m[4] = { nl_mask4(w.x), nl_mask4(w.y), nl_mask4(w.z), nl_mask4(w.w) };
+	uint32_t bits = 0;
+	#pragma unroll
+	for (int k = 0; k < 4; ++k) bits |= ((m[k] & 1) | (m[k] >> 7 & 2) | (m[k] >> 14 & 4) | (m[k] >> 21 & 8)) << (4 * k);
+	return bits;
+}
+
+__global__ void k_tiles_init(LineTileState ts, int n_tile) { ts.InitializeStatus(n_tile); }
+
+// Tiles [t_lo, t_lo + gridDim.x) of the text, one per CTA.  avail: bytes of the text present (== len unless the text is still
+// arriving, and then at least PT_TILE past the last tile of the launch).
+__global__ void __launch_bounds__(PT_THREADS)
+k_parse_tiles(const char *__restrict__ text, size_t len, size_t avail, uint64_t t_lo, unsigned *tile_ctr, LineTileState tstate,
+              int min_span, int min_match, int bi_dir, NameTab tab, PRec *out, uint64_t *start, uint64_t line_cap, unsigned long long *counts)
+{
+	typedef cub::BlockScan<uint32_t, PT_THREADS> BS;
+	__shared__ __align__(16) char s_text[PT_TILE + PT_OVER + 16];  // (+16: parse_line reads whole aligned words)
+	__shared__ uint16_t s_start[PT_LIST + 1];                      // line starts, offsets from the tile's first byte
+	__shared__ uint32_t s_vals[PT_THREADS / 32][11][32];
+	__shared__ typename BS::TempStorage s_scan;
+	__shared__ typename LinePrefixOp::TempStorage s_pref;
+	__shared__ unsigned long long s_first, s_tile, s_eol;
+	__shared__ uint32_t s_nl;
+	const uint32_t lane = threadIdx.x & 31;
+	if (threadIdx.x == 0) s_tile = t_lo + atomicAdd(tile_ctr, 1u), s_nl = ~0u;
+	__syncthreads();
+	const uint64_t t = s_tile, b0 = t * PT_TILE, b1 = b0 + PT_TILE < len ? b0 + PT_TILE : len;
+	const uint64_t w_end = b1 + PT_OVER < avail ? b1 + PT_OVER : avail;       // staged bytes: [b0, w_end)
+	{
+		const uint32_t n16 = (uint32_t)((w_end - b0 + 15) >> 4);  // the tail word may reach past `len` but stays inside the (padded) allocation
+		for (uint32_t k = threadIdx.x; k < n16; k += PT_THREADS)
+			reinterpret_cast<uint4*>(s_text)[k] = __ldg(reinterpret_cast<const uint4*>(text + b0) + k);
+	}
+	__syncthreads();
+	// newlines of this thread's 64 bytes that start a line: those before `lim` (a newline ending the text starts none)
+	const uint32_t my0 = threadIdx.x * 64, lim = (uint32_t)((b1 == len ? len - 1 : b1) - b0);
+	uint64_t bits = 0;
+	#pragma unroll
+	for (int k = 0; k < 4; ++k) bits |= (uint64_t)nl_bits_u4(reinterpret_cast<const uint4*>(s_text + my0)[k]) << (16 * k);
+	bits &= lim <= my0 ? 0ull : lim - my0 >= 64 ? ~0ull : (1ull << (lim - my0)) - 1;
+	const bool line0 = t == 0 && threadIdx.x == 0;            // line 0 starts at byte 0
+	uint32_t rank, n;
+	BS(s_scan).ExclusiveSum((uint32_t)__popcll(bits) + line0, rank, n);
+	// the tile's last line ends at the first '\n' from `lim` on (or at the end of the text)
+	for (uint32_t o = lim + threadIdx.x; o < (uint32_t)(w_end - b0); o += PT_THREADS)
+		if (s_text[o] == '\n' && b0 + o < len) { atomicMin(&s_nl, o); break; }
+	if (threadIdx.x < 32) {
+		if (t == 0) {
+			if (threadIdx.x == 0) tstate.SetInclusive(0, n), s_first = 0;
+		} else {
+			LinePrefixOp op(tstate, s_pref, ::cuda::std::plus<unsigned long long>(), (int)t);
+			const unsigned long long ex = op(n);
+			if (threadIdx.x == 0) s_first = ex;
 		}
 	}
+	__syncthreads();
+	const uint64_t first = s_first;
+	if (threadIdx.x == 0 && b1 == len) counts[PC_LINES] = first + n;
+	if (n == 0) return;
+	uint64_t last_eol = s_nl != ~0u ? b0 + s_nl : w_end >= len ? len : ~0ull; // ~0: not staged, ends past the overhang
+	if (last_eol == ~0ull) { // (the same for the whole CTA) warp 0 looks for the end of that long line in global memory
+		if (threadIdx.x < 32) {
+			uint64_t e = ~0ull;
+			for (uint64_t p = w_end; p < avail; p += 32 * 16) {
+				const uint64_t q = p + 16 * lane;
+				uint32_t m = 0;
+				for (uint32_t k = 0; k < 16 && q + k < avail; ++k) m |= (uint32_t)(text[q + k] == '\n') << k;
+				const unsigned hit = __ballot_sync(0xffffffffu, m != 0);
+				if (hit) { e = __shfl_sync(0xffffffffu, q + __ffs(m) - 1, __ffs(hit) - 1); break; }
+			}
+			if (e == ~0ull && avail == len) e = len;
+			if (threadIdx.x == 0) {
+				s_eol = e;
+				if (e == ~0ull) atomicAdd(counts + PC_CUT, 1ull); // it runs past the bytes that have arrived
+			}
+		}
+		__syncthreads();
+		last_eol = s_eol;
+	}
+	unsigned n_parsed = 0, n_pass = 0;
+	for (uint32_t r0 = 0; r0 < n; r0 += PT_LIST) {
+		{	// list the starts of the lines r0 .. r0 + PT_LIST of the tile (the last one only ends the one before it)
+			uint32_t r = rank;
+			uint64_t b = bits;
+			if (line0) { if (r == r0) s_start[0] = 0; ++r; }
+			for (; b && r <= r0 + PT_LIST; ++r, b &= b - 1)
+				if (r >= r0) s_start[r - r0] = (uint16_t)(my0 + __ffsll((long long)b));
+		}
+		__syncthreads();
+		const uint32_t cnt = n - r0 < PT_LIST ? n - r0 : PT_LIST;
+		for (uint32_t j0 = 0; j0 < cnt; j0 += PT_THREADS) {
+			const uint32_t j = j0 + threadIdx.x;
+			const uint64_t i = first + r0 + j;
+			uint32_t sq = NOSLOT, st = 0;
+			if (j < cnt && i < line_cap) {
+				const uint64_t s = b0 + s_start[j];
+				uint64_t eol = r0 + j + 1 < n ? b0 + s_start[j + 1] - 1 : last_eol;
+				if (eol != ~0ull) {
+					const char *base = eol <= w_end ? s_text - b0 : text; // base + file offset = address of that byte
+					if (eol - s > 1 && base[eol - 1] == '\r') --eol;
+					PLine r;
+					parse_line(base + s, base + eol, r, &s_vals[threadIdx.x >> 5][0][lane]);
+					if (r.nf >= 10) {
+						++n_parsed;
+						if (!(r.qe - r.qs < (uint32_t)min_span || r.te - r.ts < (uint32_t)min_span || (int)(r.ml_rev & 0x7fffffffu) < min_match)) {
+							++n_pass;
+							sq = tab_insert(tab, text, base + s, r.qnl, s, 2 * i, counts + PC_OVERFLOW);
+							st = tab_insert(tab, text, base + s + r.tdelta, r.tnl, s + r.tdelta, 2 * i + 1, counts + PC_OVERFLOW);
+						}
+					}
+					start[i] = s;
+					*reinterpret_cast<uint4*>(out + i) = make_uint4(r.qs, r.qe, r.ts, r.te);
+					*(reinterpret_cast<uint4*>(out + i) + 1) = make_uint4(r.ml_rev, (r.bl & 0x7fffffffu) | (r.nf >= 11 ? 0x80000000u : 0u), sq, st);
+				}
+			}
+			if (tab.hits) { // consecutive lines often share their query read: one add per distinct slot of the warp
+				const unsigned grp = __match_any_sync(0xffffffffu, sq);
+				if (sq != NOSLOT && lane == (uint32_t)__ffs(grp) - 1) atomicAdd(&tab.hits[sq], (uint32_t)__popc(grp));
+				if (sq != NOSLOT && bi_dir && st != sq) atomicAdd(&tab.hits[st], 1u);
+			}
+		}
+		__syncthreads(); // the list is rewritten by the next round
+	}
 	n_parsed = __reduce_add_sync(0xffffffffu, n_parsed), n_pass = __reduce_add_sync(0xffffffffu, n_pass);
-	if ((threadIdx.x & 31) == 0) {
-		if (n_parsed) atomicAdd(counts, (unsigned long long)n_parsed);
-		if (n_pass) atomicAdd(counts + 1, (unsigned long long)n_pass);
+	if (lane == 0) {
+		if (n_parsed) atomicAdd(counts + PC_PARSED, (unsigned long long)n_parsed);
+		if (n_pass) atomicAdd(counts + PC_STORED, (unsigned long long)n_pass);
 	}
 }
 
@@ -408,7 +455,8 @@ __global__ void k_nocont_mark(const PRec *ln, uint64_t n_lines, const char *text
 	}
 }
 
-__global__ void k_nocont_drop(PRec *ln, uint64_t n_lines, const uint8_t *excl, NameTab t)
+// (t.first reset to ~0 and t.hits to 0 before: both are taken again over the lines that are left)
+__global__ void k_nocont_drop(PRec *ln, uint64_t n_lines, const uint8_t *excl, int bi_dir, NameTab t)
 {
 	for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n_lines; i += (uint64_t)gridDim.x * blockDim.x) {
 		const uint32_t sq = ln[i].slot_q, st = ln[i].slot_t;
@@ -416,6 +464,8 @@ __global__ void k_nocont_drop(PRec *ln, uint64_t n_lines, const uint8_t *excl, N
 		if (excl[sq] || excl[st]) { ln[i].slot_q = NOSLOT; continue; }
 		if (t.first[sq] > 2 * i) atomicMin(&t.first[sq], (unsigned long long)(2 * i));
 		if (t.first[st] > 2 * i + 1) atomicMin(&t.first[st], (unsigned long long)(2 * i + 1));
+		atomicAdd(&t.hits[sq], 1u);
+		if (bi_dir && st != sq) atomicAdd(&t.hits[st], 1u);
 	}
 }
 
@@ -432,12 +482,15 @@ __global__ void k_dict_pairs(const uint64_t *slots, uint32_t n, NameTab t, unsig
 	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) first_out[i] = t.first[slots[i]];
 }
 
+// read_cnt[id] = hits of the read (slot -> id is a permutation: the per-slot counts of the parse become per-read counts here)
 __global__ void k_dict_rank(const unsigned long long *first_sorted, const uint64_t *slot_sorted, uint32_t n, NameTab t,
-                            const char *text, const uint64_t *start, uint64_t *noff, uint32_t *nlen, uint32_t *slen, unsigned long long *tot_len)
+                            const char *text, const uint64_t *start, uint64_t *noff, uint32_t *nlen, uint32_t *slen, unsigned long long *tot_len,
+                            uint32_t *read_cnt)
 {
 	unsigned long long sum = 0;
 	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
 		t.id[slot_sorted[i]] = i;
+		read_cnt[i] = t.hits[slot_sorted[i]];
 		occ_name(text, start, first_sorted[i], &noff[i], &nlen[i], &slen[i]); // the length kept for a read is the one of its first appearance (sdict.c:36)
 		sum += slen[i];
 	}
@@ -448,17 +501,6 @@ __global__ void k_dict_rank(const unsigned long long *first_sorted, const uint64
 }
 
 // --------------------------------------------------------------------------------------------- hits
-// hits per query read (the bucket sizes of the sort, dh_sort_buckets)
-__global__ void k_hit_count(const PRec *ln, uint64_t n_lines, int bi_dir, NameTab t, uint32_t *read_cnt)
-{
-	for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n_lines; i += (uint64_t)gridDim.x * blockDim.x) {
-		const uint2 sl = *reinterpret_cast<const uint2*>(&ln[i].slot_q);
-		if (sl.x == NOSLOT) continue;
-		atomicAdd(&read_cnt[t.id[sl.x]], 1u);
-		if (bi_dir && sl.x != sl.y) atomicAdd(&read_cnt[t.id[sl.y]], 1u);
-	}
-}
-
 // every stored line's hit, and its mirror, straight into the bucket of its query read, with the ordinal 2 * line (+ 1 for the
 // mirror) in the query-id half of qns: the order of the ordinals is the file order of the hits, as dh_sort_buckets needs
 __global__ void k_hit_emit(const PRec *ln, uint64_t n_lines, int bi_dir, NameTab t, const uint32_t *__restrict__ first, uint32_t *cur, DHit *out)
@@ -510,15 +552,7 @@ void names_free(MabDev &d, DNames &n)
 
 static inline uint32_t bits_for(uint64_t x) { uint32_t b = 0; while (x) ++b, x >>= 1; return b ? b : 1; }
 
-constexpr int SC_RNG = 40;   // d_scal[40..42]: the line range k_parse works on (lo, hi, total or ~0)
-
-static void set_rng(MabDev &d, uint64_t lo, uint64_t hi, uint64_t total)
-{
-	const unsigned long long v[3] = { lo, hi, total };
-	MAB_CUDA(cudaMemcpyAsync(d.d_scal + SC_RNG, v, sizeof(v), cudaMemcpyHostToDevice, d.stream));
-}
-
-static NameTab tab_alloc(MabDev &d, uint64_t cap)
+static NameTab tab_alloc(MabDev &d, uint64_t cap, bool with_hits)
 {
 	NameTab tab;
 	tab.key = (unsigned long long*)mab_alloc<uint64_t>(d, cap);
@@ -527,7 +561,81 @@ static NameTab tab_alloc(MabDev &d, uint64_t cap)
 	tab.mask = cap - 1;
 	MAB_CUDA(cudaMemsetAsync(tab.key, 0, cap * 8, d.stream));
 	MAB_CUDA(cudaMemsetAsync(tab.first, 0xff, cap * 8, d.stream));
+	if (with_hits) {
+		tab.hits = mab_alloc<uint32_t>(d, cap);
+		MAB_CUDA(cudaMemsetAsync(tab.hits, 0, cap * 4, d.stream));
+	}
 	return tab;
+}
+
+static void tab_free(MabDev &d, NameTab &t)
+{
+	d.free(t.key); d.free(t.first); d.free(t.id);
+	if (t.hits) d.free(t.hits);
+	t = NameTab{nullptr, nullptr, nullptr, 0};
+}
+
+// What the parse leaves: start[line], the record of every line and the dictionary of the stored lines' names.
+struct Parsed {
+	uint64_t *start = nullptr;
+	PRec *ln = nullptr;
+	NameTab tab{nullptr, nullptr, nullptr, 0};
+	uint64_t cap = 0, n_lines = 0, n_parsed = 0;
+};
+
+// Room for the lines before they are counted (a PAF line of 12 columns has at least 24 bytes) and the dictionary size
+// for it: ~50 lines name a read twice each, so the load stays <= 1/6 at that ratio; an overflow quadruples it.
+static inline uint64_t line_estimate(size_t len) { return len / 24 + 1024; }
+static inline uint64_t tab_cap_for(uint64_t line_cap) { uint64_t cap = 1ull << 20; while (cap < line_cap / 8) cap <<= 1; return cap; }
+
+// look-back state of k_parse_tiles over n_tile tiles; tiles_reset marks every tile "not done"
+static LineTileState tiles_alloc(MabDev &d, uint64_t n_tile, void **mem)
+{
+	if (n_tile >= (1ull << 31) - 64) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 tiles of PAF on one GPU\n"); exit(73); }
+	size_t bytes = 0;
+	MAB_CUDA(LineTileState::AllocationSize((int)n_tile, bytes));
+	*mem = d.alloc(bytes);
+	LineTileState ts;
+	MAB_CUDA(ts.Init((int)n_tile, *mem, bytes));
+	return ts;
+}
+
+static void tiles_reset(MabDev &d, LineTileState ts, uint64_t n_tile)
+{
+	MAB_LAUNCH(d, k_tiles_init, mab_grid(n_tile, 256, 1u << 30), 256, 0, ts, (int)n_tile);
+}
+
+// The whole text is resident: one launch over all tiles, with no host synchronisation before it.  start and ln are sized from
+// the estimate; a text with more lines, or with more names than the dictionary holds, is parsed again with room for all of them.
+static void parse_resident(MabDev &d, const char *d_text, size_t len, int min_span, int min_match, int bi_dir, bool count_hits, Parsed &p)
+{
+	const uint64_t n_tile = (len + PT_TILE - 1) / PT_TILE;
+	uint64_t line_cap = line_estimate(len), cap = tab_cap_for(line_cap);
+	unsigned *ctr = mab_alloc<unsigned>(d, 1);
+	void *ts_mem = nullptr;
+	const LineTileState ts = tiles_alloc(d, n_tile, &ts_mem);
+	for (;;) {
+		p.start = mab_alloc<uint64_t>(d, line_cap);
+		p.ln = mab_alloc<PRec>(d, line_cap);
+		p.tab = tab_alloc(d, cap, count_hits);
+		d.zero_scal(SC_COUNT, PC_N);
+		if (n_tile) {
+			tiles_reset(d, ts, n_tile);
+			MAB_CUDA(cudaMemsetAsync(ctr, 0, 4, d.stream));
+			MAB_LAUNCH(d, k_parse_tiles, (unsigned)n_tile, PT_THREADS, 0, d_text, len, len, 0, ctr, ts, min_span, min_match, bi_dir, p.tab, p.ln, p.start,
+			           line_cap, d.d_scal + SC_COUNT);
+		}
+		p.n_parsed = d.get_scal(SC_COUNT + PC_PARSED);
+		p.n_lines = d.h_scal[SC_COUNT + PC_LINES];
+		const bool more_lines = p.n_lines > line_cap, overflow = d.h_scal[SC_COUNT + PC_OVERFLOW] != 0;
+		if (!more_lines && !overflow) break;
+		d.free(p.start); d.free(p.ln); tab_free(d, p.tab);
+		if (more_lines) line_cap = p.n_lines;
+		if (overflow) cap <<= 2;
+		if (cap > (1ull << 33)) { fprintf(stderr, "[E::miniasm_b200] read-name table overflow\n"); exit(77); }
+	}
+	d.free(ctr); d.free(ts_mem);
+	p.cap = cap;
 }
 
 static void ingest_finish(MabDev &d, const char *d_text, size_t len, uint64_t *start, PRec *ln, uint64_t n_lines, NameTab tab, uint64_t cap, int bi_dir,
@@ -540,93 +648,68 @@ void ingest_paf(MabDev &d, const char *d_text, size_t len, int min_span, int min
 	names = DNames();
 	h.n = 0, h.n_seq = 0;
 	if (len == 0) { dh_reserve(d, h, 1); return; }
+	if (len >= (1ull << NT_OFF_BITS) - 1) { fprintf(stderr, "[E::miniasm_b200] more than 2^37 bytes of PAF on one GPU\n"); exit(73); }
 
 	d.trace("ingest:begin");
-	// (1) line starts: count newlines per 16 KB tile, scan the tile counts, write the positions
-	uint64_t n_lines;
-	uint64_t *start = dev_line_starts(d, d_text, len, &n_lines);
-	st.n_lines = n_lines;
-	d.trace("ingest:line_starts");
-
-	// (2) parse + store filter + dictionary insert in one pass; the table grows (and the pass repeats) until every name has a slot
-	if (len >= (1ull << NT_OFF_BITS) - 1) { fprintf(stderr, "[E::miniasm_b200] more than 2^37 bytes of PAF on one GPU\n"); exit(73); }
-	PRec *ln = mab_alloc<PRec>(d, n_lines);
-	NameTab tab{nullptr, nullptr, nullptr, 0};
-	uint64_t cap = 1ull << 20;
-	while (cap < n_lines / 4) cap <<= 1;                 // ~50 lines name a read twice each: load <= 1/6 at that ratio; overflow quadruples it
-	for (;;) {
-		tab = tab_alloc(d, cap);
-		d.zero_scal(SC_COUNT, 4);
-		set_rng(d, 0, n_lines, n_lines);
-		MAB_LAUNCH(d, k_parse, mab_grid((n_lines + PARSE_LINES - 1) / PARSE_LINES, 1, MAB_SMS * 16u), PARSE_LINES, 0, d_text, len, start, d.d_scal + SC_RNG, min_span, min_match, tab, ln, d.d_scal + SC_COUNT);
-		st.n_parsed = d.get_scal(SC_COUNT);
-		if (d.h_scal[SC_COUNT + 2] == 0) break;
-		d.free(tab.key); d.free(tab.first); d.free(tab.id);
-		cap <<= 2;
-		if (cap > (1ull << 33)) { fprintf(stderr, "[E::miniasm_b200] read-name table overflow\n"); exit(77); }
-	}
-	ingest_finish(d, d_text, len, start, ln, n_lines, tab, cap, bi_dir, nocont, h, names, st);
+	// (1)+(2) line starts, parse, store filter, dictionary insert and hit counts per name in one pass
+	Parsed p;
+	parse_resident(d, d_text, len, min_span, min_match, bi_dir, true, p);
+	st.n_parsed = p.n_parsed, st.n_lines = p.n_lines;
+	d.trace("ingest:parse");
+	ingest_finish(d, d_text, len, p.start, p.ln, p.n_lines, p.tab, p.cap, bi_dir, nocont, h, names, st);
 }
 
-// Front end of an ingest with the text still on the host: it crosses PCIe in 64 MB chunks on a copy stream while the chunks that
-// have arrived are scanned for line starts and parsed (store filter, dictionary) on the context's stream -- k_parse needs nothing
-// global any more.  host_text may be pageable or pinned (pinned overlaps fully); d_text has room for len + 64.  Capacities are
-// estimates (a 12-column line has >= 24 bytes): false = the text broke them (or the dictionary overflowed), nothing is kept and the
-// caller parses the now-resident text the plain way.  No collectives inside (the sharded ingest calls it rank by rank).
-static bool stream_parse(MabDev &d, char *d_text, const char *host_text, size_t len, int min_span, int min_match,
-                         uint64_t **start_out, PRec **ln_out, NameTab *tab_out, uint64_t *cap_out, uint64_t *n_lines_out, uint64_t *n_parsed_out)
+// Front end of an ingest with the text still on the host: it crosses PCIe in 64 MB chunks on a copy stream while the tiles that
+// have arrived are parsed (line starts, store filter, dictionary) on the context's stream, one launch of k_parse_tiles per chunk.
+// The look-back state lives across the launches; the last tile that has arrived waits for the next chunk, so every parsed tile
+// has its overhang.  host_text may be pageable or pinned (pinned overlaps fully); d_text has room for len + 64.  Capacities are
+// estimates: false = the text broke them (more lines than estimated, more names than slots, or a line that runs past a chunk),
+// nothing is kept and the caller parses the now-resident text the plain way.  No collectives inside (the sharded ingest calls it
+// rank by rank).
+static bool stream_parse(MabDev &d, char *d_text, const char *host_text, size_t len, int min_span, int min_match, int bi_dir, bool count_hits, Parsed &p)
 {
-	const uint64_t CH_TILES = (64ull << 20) / NL_TILE, n_tile = (len + NL_TILE - 1) / NL_TILE;       // 64 MB chunks, whole tiles
+	const uint64_t CH_TILES = (64ull << 20) / PT_TILE, n_tile = (len + PT_TILE - 1) / PT_TILE;       // 64 MB chunks, whole tiles
 	const uint64_t n_chunk = (n_tile + CH_TILES - 1) / CH_TILES;
-	const uint64_t line_cap = len / 24 + 1024;
-	uint64_t cap = 1ull << 20;
-	while (cap < line_cap / 8) cap <<= 1;
-	uint64_t *start = mab_alloc<uint64_t>(d, line_cap + 1);
-	PRec *ln = mab_alloc<PRec>(d, line_cap);
-	uint64_t *cnt = mab_alloc<uint64_t>(d, CH_TILES + 1), *base = mab_alloc<uint64_t>(d, CH_TILES + 1);
-	unsigned long long *state = (unsigned long long*)mab_alloc<uint64_t>(d, 8);   // [0] newline-started lines seen, [1] capacity; [4..6] = rng
-	NameTab tab = tab_alloc(d, cap);
-	{
-		const unsigned long long init[8] = { 0, line_cap, 0, 0, 0, 0, ~0ull, 0 };
-		MAB_CUDA(cudaMemcpyAsync(state, init, sizeof(init), cudaMemcpyHostToDevice, d.stream));
-		MAB_CUDA(cudaMemsetAsync(start, 0, 8, d.stream));
-	}
-	d.zero_scal(SC_COUNT, 4);
-	size_t tb = 0;
-	cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt, base, (int64_t)CH_TILES, d.stream);
-	void *tmp = d.tmp(tb);
+	const uint64_t line_cap = line_estimate(len), cap = tab_cap_for(line_cap);
+	p.start = mab_alloc<uint64_t>(d, line_cap);
+	p.ln = mab_alloc<PRec>(d, line_cap);
+	p.tab = tab_alloc(d, cap, count_hits);
+	unsigned *ctr = mab_alloc<unsigned>(d, n_chunk);                // tile counter of each launch
+	MAB_CUDA(cudaMemsetAsync(ctr, 0, n_chunk * 4, d.stream));
+	void *ts_mem = nullptr;
+	const LineTileState ts = tiles_alloc(d, n_tile, &ts_mem);
+	tiles_reset(d, ts, n_tile);
+	d.zero_scal(SC_COUNT, PC_N);
 	if (!d.copy_stream) MAB_CUDA(cudaStreamCreateWithFlags(&d.copy_stream, cudaStreamNonBlocking));
 	std::vector<cudaEvent_t> ev(n_chunk);
 	cudaEvent_t ready;
 	MAB_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
 	MAB_CUDA(cudaEventRecord(ready, d.stream));                 // the copies may not overtake whatever still uses d_text on the main stream
 	MAB_CUDA(cudaStreamWaitEvent(d.copy_stream, ready, 0));
-	for (uint64_t k = 0; k < n_chunk; ++k) { // copy k is issued before the kernels of chunk k: a pageable source blocks the host per chunk, not for the whole text
+	uint64_t t_done = 0;                                         // tiles [0, t_done) are parsed
+	for (uint64_t k = 0; k < n_chunk; ++k) { // copy k is issued before the kernel of chunk k: a pageable source blocks the host per chunk, not for the whole text
 		const uint64_t t0 = k * CH_TILES, t1 = (k + 1) * CH_TILES < n_tile ? (k + 1) * CH_TILES : n_tile;
-		const uint64_t b0 = t0 * NL_TILE, b1 = t1 * NL_TILE < len ? t1 * NL_TILE : len;
+		const uint64_t b0 = t0 * PT_TILE, b1 = t1 * PT_TILE < len ? t1 * PT_TILE : len;
 		MAB_CUDA(cudaEventCreateWithFlags(&ev[k], cudaEventDisableTiming));
 		MAB_CUDA(cudaMemcpyAsync(d_text + b0, host_text + b0, b1 - b0, cudaMemcpyHostToDevice, d.copy_stream));
 		MAB_CUDA(cudaEventRecord(ev[k], d.copy_stream));
 		MAB_CUDA(cudaStreamWaitEvent(d.stream, ev[k], 0));
-		MAB_LAUNCH(d, k_nl_count_range, mab_grid(t1 - t0, 1, MAB_SMS * 8u), NL_THREADS, 0, d_text, len, t0, t1, cnt);
-		cub::DeviceScan::ExclusiveSum(tmp, tb, cnt, base, (int64_t)(t1 - t0), d.stream);
-		++d.n_lib;
-		MAB_LAUNCH(d, k_nl_write_range, mab_grid(t1 - t0, 1, MAB_SMS * 8u), NL_THREADS, 0, d_text, len, t0, t1, base, state, start);
-		MAB_LAUNCH(d, k_nl_advance, 1, 32, 0, state, base, cnt, t1 - t0, state + 4, (int)(k + 1 == n_chunk));
-		MAB_LAUNCH(d, k_parse, MAB_SMS * 8u, PARSE_LINES, 0, d_text, len, start, state + 4, min_span, min_match, tab, ln, d.d_scal + SC_COUNT);
+		const uint64_t t_hi = k + 1 == n_chunk ? n_tile : t1 - 1;
+		MAB_LAUNCH(d, k_parse_tiles, (unsigned)(t_hi - t_done), PT_THREADS, 0, d_text, len, b1, t_done, ctr + k, ts, min_span, min_match, bi_dir, p.tab, p.ln,
+		           p.start, line_cap, d.d_scal + SC_COUNT);
+		t_done = t_hi;
 	}
-	unsigned long long fin[8];
-	MAB_CUDA(cudaMemcpyAsync(fin, state, sizeof(fin), cudaMemcpyDeviceToHost, d.stream));
-	*n_parsed_out = d.get_scal(SC_COUNT);                       // (synchronises)
+	p.n_parsed = d.get_scal(SC_COUNT + PC_PARSED);               // (synchronises)
 	for (uint64_t k = 0; k < n_chunk; ++k) MAB_CUDA(cudaEventDestroy(ev[k]));
 	MAB_CUDA(cudaEventDestroy(ready));
-	d.free(cnt); d.free(base); d.free(state);
-	const uint64_t n_lines = fin[0] + 1;
-	if (n_lines >= line_cap || d.h_scal[SC_COUNT + 2] != 0) {   // estimates broken (very short lines / more names than slots)
-		d.free(start); d.free(ln); d.free(tab.key); d.free(tab.first); d.free(tab.id);
+	d.free(ctr); d.free(ts_mem);
+	p.n_lines = d.h_scal[SC_COUNT + PC_LINES];
+	if (p.n_lines > line_cap || d.h_scal[SC_COUNT + PC_OVERFLOW] != 0 || d.h_scal[SC_COUNT + PC_CUT] != 0) {
+		d.free(p.start); d.free(p.ln); tab_free(d, p.tab);
+		p = Parsed();
 		return false;
 	}
-	*start_out = start, *ln_out = ln, *tab_out = tab, *cap_out = cap, *n_lines_out = n_lines;
+	p.cap = cap;
 	return true;
 }
 
@@ -640,14 +723,14 @@ void ingest_paf_stream(MabDev &d, char *d_text, const char *host_text, size_t le
 	h.n = 0, h.n_seq = 0;
 	if (len == 0) { dh_reserve(d, h, 1); return; }
 	if (len >= (1ull << NT_OFF_BITS) - 1) { fprintf(stderr, "[E::miniasm_b200] more than 2^37 bytes of PAF on one GPU\n"); exit(73); }
-	uint64_t *start; PRec *ln; NameTab tab; uint64_t cap, n_lines, n_parsed;
-	if (!stream_parse(d, d_text, host_text, len, min_span, min_match, &start, &ln, &tab, &cap, &n_lines, &n_parsed)) {
-		ingest_paf(d, d_text, len, min_span, min_match, bi_dir, h, names, st, nullptr); // the text is resident now: the plain path sizes exactly
+	Parsed p;
+	if (!stream_parse(d, d_text, host_text, len, min_span, min_match, bi_dir, true, p)) {
+		ingest_paf(d, d_text, len, min_span, min_match, bi_dir, h, names, st, nullptr); // the text is resident now: the plain path parses it again
 		return;
 	}
-	st.n_parsed = n_parsed, st.n_lines = n_lines;
-	d.trace("ingest:stream (copy + line starts + parse + dictionary)");
-	ingest_finish(d, d_text, len, start, ln, n_lines, tab, cap, bi_dir, nullptr, h, names, st);
+	st.n_parsed = p.n_parsed, st.n_lines = p.n_lines;
+	d.trace("ingest:stream (copy + parse + dictionary + hit counts)");
+	ingest_finish(d, d_text, len, p.start, p.ln, p.n_lines, p.tab, p.cap, bi_dir, nullptr, h, names, st);
 }
 
 static void ingest_finish(MabDev &d, const char *d_text, size_t len, uint64_t *start, PRec *ln, uint64_t n_lines, NameTab tab, uint64_t cap, int bi_dir,
@@ -663,12 +746,13 @@ static void ingest_finish(MabDev &d, const char *d_text, size_t len, uint64_t *s
 		d.zero_scal(SC_AUX, 1);
 		MAB_LAUNCH(d, k_count_u8, mab_grid(cap, 256), 256, 0, excl, cap, d.d_scal + SC_AUX);
 		MAB_CUDA(cudaMemsetAsync(tab.first, 0xff, cap * 8, d.stream));
-		MAB_LAUNCH(d, k_nocont_drop, mab_grid(n_lines, 256), 256, 0, ln, n_lines, excl, tab);
+		MAB_CUDA(cudaMemsetAsync(tab.hits, 0, cap * 4, d.stream));
+		MAB_LAUNCH(d, k_nocont_drop, mab_grid(n_lines, 256), 256, 0, ln, n_lines, excl, bi_dir, tab);
 		st.n_dropped = d.get_scal(SC_AUX);
 		d.free(excl);
 		d.trace("ingest:-R prefilter");
 	}
-	// (4) ids = rank of the first occurrence
+	// (4) ids = rank of the first occurrence; the hit counts of the slots become those of the reads (the bucket sizes of the sort)
 	uint64_t *slots = mab_alloc<uint64_t>(d, cap);
 	uint32_t n_seq;
 	{
@@ -686,6 +770,8 @@ static void ingest_finish(MabDev &d, const char *d_text, size_t len, uint64_t *s
 	}
 	names.n_seq = n_seq;
 	names.off = mab_alloc<uint64_t>(d, n_seq); names.nlen = mab_alloc<uint32_t>(d, n_seq); names.slen = mab_alloc<uint32_t>(d, n_seq);
+	uint32_t *read_cnt = mab_alloc<uint32_t>(d, (size_t)n_seq + 1), *first = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);
+	MAB_CUDA(cudaMemsetAsync(read_cnt + n_seq, 0, 4, d.stream));
 	if (n_seq) {
 		unsigned long long *fa = (unsigned long long*)mab_alloc<uint64_t>(d, n_seq), *fb = (unsigned long long*)mab_alloc<uint64_t>(d, n_seq);
 		uint64_t *sb = mab_alloc<uint64_t>(d, n_seq);
@@ -699,17 +785,15 @@ static void ingest_finish(MabDev &d, const char *d_text, size_t len, uint64_t *s
 		cub::DeviceRadixSort::SortPairs(tmp, tb, dk, dv, (int)n_seq, 0, end_bit, d.stream);
 		++d.n_lib;
 		d.zero_scal(SC_AUX, 1);
-		MAB_LAUNCH(d, k_dict_rank, mab_grid(n_seq, 256), 256, 0, dk.Current(), dv.Current(), n_seq, tab, d_text, start, names.off, names.nlen, names.slen, d.d_scal + SC_AUX);
+		MAB_LAUNCH(d, k_dict_rank, mab_grid(n_seq, 256), 256, 0, dk.Current(), dv.Current(), n_seq, tab, d_text, start, names.off, names.nlen, names.slen, d.d_scal + SC_AUX,
+		           read_cnt);
 		st.tot_len = d.get_scal(SC_AUX);
 		d.free(fa); d.free(fb); d.free(sb);
 	}
 	d.free(slots);
 
 	d.trace("ingest:rank_ids");
-	// (5) hits counted per query read, then emitted straight into their read's bucket of h.a2
-	uint32_t *read_cnt = mab_alloc<uint32_t>(d, (size_t)n_seq + 1), *first = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);
-	MAB_CUDA(cudaMemsetAsync(read_cnt, 0, ((size_t)n_seq + 1) * 4, d.stream));
-	MAB_LAUNCH(d, k_hit_count, mab_grid(n_lines, 256), 256, 0, ln, n_lines, bi_dir, tab, read_cnt);
+	// (5) every hit emitted straight into its read's bucket of h.a2
 	dh_bucket_first(d, read_cnt, n_seq, first);
 	MAB_CUDA(cudaMemsetAsync(read_cnt, 0, (size_t)n_seq * 4, d.stream)); // the counts become the buckets' fill cursors
 	uint32_t n_hits;
@@ -720,7 +804,7 @@ static void ingest_finish(MabDev &d, const char *d_text, size_t len, uint64_t *s
 	if (n_hits) MAB_LAUNCH(d, k_hit_emit, mab_grid(n_lines, 256), 256, 0, ln, n_lines, bi_dir, tab, first, read_cnt, h.a2);
 	st.n_hits = n_hits, st.n_seq = n_seq;
 	d.free(ln); d.free(start);
-	d.free(tab.key); d.free(tab.first); d.free(tab.id);
+	tab_free(d, tab);
 
 	d.trace("ingest:emit_hits");
 	// (6) ma_hit_sort: order every bucket (h.a2 -> h.a)
@@ -1005,40 +1089,16 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 	const int G = sc.world;
 	// (1)+(2) local line starts, parse + store filter + local dictionary (exact: occurrences are compared with a witness in the text)
 	if (len >= (1ull << NT_OFF_BITS) - 1) { fprintf(stderr, "[E::miniasm_b200] more than 2^37 bytes of PAF on one GPU\n"); exit(73); }
-	uint64_t *start = nullptr, n_lines = 0, cap = 1ull << 20, n_parsed = 0;
-	PRec *ln = nullptr;
-	NameTab tab{nullptr, nullptr, nullptr, 0};
+	Parsed p;
 	bool have = false;                                      // this rank holds a finished local parse
 	if (host_text && len) {
-		have = stream_parse(d, d_text, host_text, len, min_span, min_match, &start, &ln, &tab, &cap, &n_lines, &n_parsed);
-		if (!have) cap = 1ull << 20;
-		d.trace("shard-ingest:stream (copy + line starts + parse + dictionary)");
+		have = stream_parse(d, d_text, host_text, len, min_span, min_match, bi_dir, false, p);
+		d.trace("shard-ingest:stream (copy + parse + dictionary)");
 	}
-	if (!have) {
-		if (len) start = dev_line_starts(d, d_text, len, &n_lines);
-		ln = mab_alloc<PRec>(d, n_lines);
-		while (cap < n_lines / 4) cap <<= 1;
-	}
-	for (;;) {
-		bool overflow = false;
-		if (!have) {
-			tab = tab_alloc(d, cap);
-			d.zero_scal(SC_COUNT, 4);
-			set_rng(d, 0, n_lines, n_lines);
-			if (n_lines) MAB_LAUNCH(d, k_parse, mab_grid((n_lines + PARSE_LINES - 1) / PARSE_LINES, 1, MAB_SMS * 16u), PARSE_LINES, 0, d_text, len, start, d.d_scal + SC_RNG, min_span, min_match, tab, ln, d.d_scal + SC_COUNT);
-			n_parsed = d.get_scal(SC_COUNT);
-			overflow = d.h_scal[SC_COUNT + 2] != 0;
-		}
-		// every rank must take the same branch: agree on the outcome
-		std::vector<uint64_t> f = sc_allgather_u64(d, sc, overflow);
-		bool any = false;
-		for (int r = 0; r < G; ++r) any |= f[r] != 0;
-		if (!any) break;
-		d.free(tab.key); d.free(tab.first); d.free(tab.id);   // (a rank whose own table was fine parses again too: same branch everywhere)
-		have = false;
-		cap <<= 2;
-		if (cap > (1ull << 33)) { fprintf(stderr, "[E::miniasm_b200] read-name table overflow\n"); exit(77); }
-	}
+	if (!have) parse_resident(d, d_text, len, min_span, min_match, bi_dir, false, p); // (local: the dictionary grows on this rank alone)
+	uint64_t *start = p.start, n_lines = p.n_lines, cap = p.cap, n_parsed = p.n_parsed;
+	PRec *ln = p.ln;
+	NameTab tab = p.tab;
 	st.n_parsed = n_parsed;
 	std::vector<uint64_t> all_lines = sc_allgather_u64(d, sc, n_lines);
 	uint64_t line_base = 0, n_lines_all = 0;
@@ -1284,7 +1344,7 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 	d.trace("shard-ingest:exchange");
 	d.sync();
 	d.free(ln); d.free(start);
-	d.free(tab.key); d.free(tab.first); d.free(tab.id);
+	tab_free(d, tab);
 	d.free(gt.key); d.free(gt.first); d.free(gt.win); d.free(gt.id);
 	d.free(g_ent); d.free(g_pos); d.free(slots); d.free(slot_of);
 	std::vector<uint64_t> hits_all = sc_allgather_u64(d, sc, n_recv), parsed_all = sc_allgather_u64(d, sc, st.n_parsed);
