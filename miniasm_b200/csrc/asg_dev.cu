@@ -112,6 +112,22 @@ __global__ void k_arc_count_dead(ArcKeep keep, uint32_t n, unsigned long long *n
 	if ((threadIdx.x & 31) == 0 && dead) atomicAdd(n_dead, (unsigned long long)dead);
 }
 
+__global__ void k_seq_count_del(const uint32_t *seq, uint32_t n, unsigned long long *n_del)
+{
+	unsigned c = 0;
+	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) c += seq[i] >> 31;
+	c = __reduce_add_sync(0xffffffffu, c);
+	if ((threadIdx.x & 31) == 0 && c) atomicAdd(n_del, (unsigned long long)c);
+}
+
+uint32_t dg_n_del_seq(MabDev &d, const DGraph &g)
+{
+	if (g.n_seq == 0) return 0;
+	d.zero_scal(SC_NSEL);
+	MAB_LAUNCH(d, k_seq_count_del, mab_grid(g.n_seq, 256), 256, 0, g.seq, g.n_seq, d.d_scal + SC_NSEL);
+	return (uint32_t)d.get_scal(SC_NSEL);
+}
+
 void dg_arc_rm(MabDev &d, DGraph &g, const uint8_t *flag)
 {
 	if (g.n_arc == 0) return;

@@ -21,6 +21,7 @@ void dg_free(MabDev &d, DGraph &g);
 
 // asg.c:57-70 (+ optional external deletion flags produced by dg_del_trans)
 void dg_arc_rm(MabDev &d, DGraph &g, const uint8_t *flag);
+uint32_t dg_n_del_seq(MabDev &d, const DGraph &g); // reads with the del bit set
 void dg_arc_sort(MabDev &d, DGraph &g);          // asg.c:22-25
 void dg_build_sorted(MabDev &d, DGraph &g, uint64_t *key, uint64_t *val, uint64_t *key2, uint64_t *val2, uint32_t n_in, uint32_t n_real, uint32_t lb, bool has_sentinel);
 void dg_arc_index(MabDev &d, DGraph &g);         // asg.c:27-42

@@ -886,7 +886,7 @@ int mab_layout_sharded(mab_ctx_t *c, const ma_opt_t *opt)
 	std::vector<const DArc*> peer_ptr((size_t)G, nullptr);
 	for (int r = 0; r < G; ++r) peer_ptr[r] = (const DArc*)peer_any[r];
 	if (p2p) {
-		dg_arc_index(d, loc);                                   // slabs of the vertices this rank owns
+		if (!loc.has_idx) dg_arc_index(d, loc);                 // slabs of the vertices this rank owns
 		uint64_t *nidx = mab_alloc<uint64_t>(d, (size_t)n * 2);
 		if (n) MAB_CUDA(cudaMemcpyAsync(nidx, loc.idx, (size_t)n * 16, cudaMemcpyDeviceToDevice, d.stream));
 		sc_allreduce(d, sc, nidx, (size_t)n * 2, ncclUint64, ncclSum); // every vertex is indexed by exactly one rank

@@ -468,13 +468,17 @@ void dh_sort(MabDev &d, DHits &h)
 // end of their group), one device-wide radix sort orders all groups at once, then one warp per group
 // sweeps its 2*count keys with a warp scan.
 // ---------------------------------------------------------------------------------------------
-__global__ void k_group_bounds(const DHit *a, size_t n, uint32_t *g32)
+// unsorted != null: set when the query ids do not ascend (the bounds are then meaningless)
+__global__ void k_group_bounds(const DHit *a, size_t n, uint32_t *g32, unsigned long long *unsorted)
 {
+	bool bad = false;
 	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-		uint32_t q = (uint32_t)(a[i].qns >> 32);
-		if (i == 0 || (uint32_t)(a[i - 1].qns >> 32) != q) g32[2 * (size_t)q + 1] = (uint32_t)i;
+		uint32_t q = (uint32_t)(a[i].qns >> 32), prev = i ? (uint32_t)(a[i - 1].qns >> 32) : 0;
+		if (i == 0 || prev != q) g32[2 * (size_t)q + 1] = (uint32_t)i;
 		if (i == n - 1 || (uint32_t)(a[i + 1].qns >> 32) != q) g32[2 * (size_t)q] = (uint32_t)(i + 1);
+		bad |= i && prev > q;
 	}
+	if (bad && unsorted) *unsorted = 1ull;
 }
 
 // Slots at or past their read's bound (grp) are dead: dh_select leaves them behind the live hits of each bucket, still under
@@ -859,7 +863,7 @@ uint64_t dh_sub(MabDev &d, const DHits &h, int min_dp, float min_iden, int end_c
 		if (!grp) {
 			grp = mab_alloc<uint64_t>(d, n_seq);
 			MAB_CUDA(cudaMemsetAsync(grp, 0, (size_t)n_seq * 8, d.stream));
-			MAB_LAUNCH(d, k_group_bounds, mab_grid(h.n, 256), 256, 0, h.a, h.n, (uint32_t*)grp);
+			MAB_LAUNCH(d, k_group_bounds, mab_grid(h.n, 256), 256, 0, h.a, h.n, (uint32_t*)grp, nullptr);
 		}
 		uint32_t *big = mab_alloc<uint32_t>(d, n_seq);
 		MAB_CUDA(cudaMemsetAsync(d.d_scal, 0, 8 * sizeof(unsigned long long), d.stream));
@@ -1242,11 +1246,12 @@ k_sel_final_count(const uint64_t *__restrict__ grp, const uint32_t *__restrict__
 	}
 }
 
-// renumber the surviving hits of each kept read and write them densely at off[new id]; also reports the new read count
-// (*n_new) and hit count to scal
+// renumber the surviving hits of each kept read and write them densely at off[new id], with their bounds in grp_out[new id]
+// (a fresh array: other warps still read grp[r] of old ids r >= m); also reports the new read count (*n_new) and hit count to scal
 __global__ void __launch_bounds__(256)
 k_sel_final_copy(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const int32_t *__restrict__ map, uint32_t n_seq,
-                 const uint32_t *__restrict__ off, const uint32_t *__restrict__ n_new, DHit *__restrict__ out, unsigned long long *scal)
+                 const uint32_t *__restrict__ off, const uint32_t *__restrict__ n_new, DHit *__restrict__ out, uint64_t *__restrict__ grp_out,
+                 unsigned long long *scal)
 {
 	const int lane = threadIdx.x & 31;
 	const unsigned lt = (1u << lane) - 1u;
@@ -1254,6 +1259,7 @@ k_sel_final_copy(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, c
 	for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_seq; r += (gridDim.x * blockDim.x) >> 5) {
 		const int32_t m = map[r];
 		if (m < 0) continue;
+		if (lane == 0) { const uint32_t s = off[m], e = off[m + 1]; grp_out[m] = e > s ? (uint64_t)s << 32 | e : 0; }
 		const uint64_t g = grp[r];
 		const uint32_t end = (uint32_t)g, first = (uint32_t)(g >> 32);
 		if (end == 0) continue;
@@ -1295,7 +1301,7 @@ size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t 
 	if (!h.grp) { // hits that did not come through the sort (mab_load_hits): the bounds of their runs
 		h.grp = mab_alloc<uint64_t>(d, n_seq);
 		MAB_CUDA(cudaMemsetAsync(h.grp, 0, (size_t)n_seq * 8, d.stream));
-		if (h.n) MAB_LAUNCH(d, k_group_bounds, mab_grid(h.n, 256), 256, 0, h.a, h.n, (uint32_t*)h.grp);
+		if (h.n) MAB_LAUNCH(d, k_group_bounds, mab_grid(h.n, 256), 256, 0, h.a, h.n, (uint32_t*)h.grp, nullptr);
 	}
 	dh_sub(d, h, o.min_dp, o.min_iden, 0, sub);
 	if (hk.sub_done) hk.sub_done(sub);
@@ -1347,7 +1353,8 @@ size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t 
 	MAB_LAUNCH(d, k_cont_map, mab_grid(n_seq, 256), 256, 0, n_seq, keep, excl, map_out, sub, sub2);
 	MAB_LAUNCH(d, k_sel_final_count, warp_grid(n_seq, 8), 256, 0, h.grp, tn, map_out, n_seq, cnt); // cnt[0 ..< reads kept]
 	exclusive_sum(d, cnt, off, (size_t)n_seq + 1);      // off[reads kept] = hits kept; later entries are not used
-	MAB_LAUNCH(d, k_sel_final_copy, warp_grid(n_seq, 8), 256, 0, h.a, h.grp, map_out, n_seq, off, excl + n_seq, h.a2, d.d_scal);
+	uint64_t *grp_new = mab_alloc<uint64_t>(d, n_seq);
+	MAB_LAUNCH(d, k_sel_final_copy, warp_grid(n_seq, 8), 256, 0, h.a, h.grp, map_out, n_seq, off, excl + n_seq, h.a2, grp_new, d.d_scal);
 	const uint32_t n_new = (uint32_t)d.get_scal(SCS_NSEQ);
 	const size_t n_hits = (size_t)d.h_scal[SCS_NHITS];
 	const unsigned long long n_cut2 = d.h_scal[SCS_CUT2];
@@ -1355,7 +1362,8 @@ size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t 
 	d.free(sub2); d.free(used); d.free(keep); d.free(excl); d.free(cnt); d.free(off);
 	DHit *t = h.a; h.a = h.a2; h.a2 = t;
 	h.n = n_hits, h.n_seq = n_new;
-	drop_bounds(d, h);
+	d.free(h.grp);
+	h.grp = grp_new;
 	d.trace("select:cut2+contained");
 
 	unsigned long long gv[2] = { n_cut2, (unsigned long long)h.n };
@@ -1409,82 +1417,84 @@ __global__ void k_sg_arcs(const DHit *a, size_t n, uint32_t *seq, HitArcParams p
 
 // ---------------------------------------------------------------------------------------------
 // ma_sg_gen without a device-wide sort (the default; MAB_SG_SEGSORT=0 or a case it declines -> the column sort above).
-// Hits arrive grouped by query read, and an arc's source vertex is its hit's query, so asg.c's "append, then sort by
-// ul" only has to order each read's arcs by (direction, length), hit order on ties -- a per-read problem of ~100
-// elements.  Pass 1 classifies every hit (flag byte, group bounds, the deletion side effects of asm.c:27-33) and
-// checks that query ids ascend; a scan of the flags gives each read its output offset; pass 2 re-classifies a read's
-// hits (cheaper than storing 16 B per hit), sorts the keys ((dir << lb | len) << 9 | arc number) with the register
-// network of ma_hit_sub and writes the read's arcs in place.  Reads with 257..8192 hits take a CTA and a shared-memory
-// network; anything the scheme cannot take (unsorted ids, a read beyond 8192 hits, reads longer than 4 Mb) falls
-// back to the column sort, so results never depend on the switch.
+// Hits arrive grouped by query read (h.grp), and an arc's source vertex is its hit's query, so asg.c's "append, then sort
+// by ul" only has to order each read's arcs by (direction, length), hit order on ties -- a per-read problem of ~100
+// elements.  One pass over the hits: a CTA takes the next tile of SGW_WARPS consecutive reads, and each warp classifies
+// its read's hits (with the deletion side effects of asm.c:27-33, which only ever set the read's own seq word) and sorts
+// the keys ((dir << lb | len) << 9 | arc number) with the register network of ma_hit_sub.  The tile's arc count gets its
+// offset from a decoupled look-back over the tiles before it (tiles start in order, so it never waits on one that is not
+// running), and each warp writes its read's arcs and both index words: the sort puts direction 0 first, so the two slab
+// lengths are the direction counts.  A read of 257..8192 hits is only counted by its warp, which reserves its arcs in the
+// tile; a CTA with a shared-memory network sorts and writes it afterwards.  What the scheme cannot take (unsorted ids, a
+// read beyond 8192 hits, reads longer than 4 Mb) is found before the launch and goes to the column sort, so results never
+// depend on the switch.
 // ---------------------------------------------------------------------------------------------
 constexpr int SGW_WARPS = 8, SGW_HITS = 256, SGW_IDX_BITS = 9;
-constexpr int SGC_HITS = 8192;
+constexpr int SGC_HITS = 8192, SGC_THREADS = 512;
 
-__global__ void k_sg_classify(const DHit *a, size_t n, uint32_t *seq, HitArcParams p, uint8_t *emit_flag, uint32_t *g32, unsigned long long *scal)
+typedef cub::ScanTileState<uint32_t> ArcTileState;
+typedef cub::TilePrefixCallbackOp<uint32_t, ::cuda::std::plus<uint32_t>, ArcTileState> ArcPrefixOp;
+
+__global__ void k_arc_tiles_init(ArcTileState ts, int n_tile) { ts.InitializeStatus(n_tile); }
+
+__global__ void k_grp_max(const uint64_t *grp, uint32_t n, unsigned long long *mx)
 {
-	unsigned cnt = 0;
-	bool bad = false;
-	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-		DHit h = ld_hit(a + i);
-		const uint32_t qn = (uint32_t)(h.qns >> 32);
-		DArc t;
-		t.ul = 0, t.v = 0, t.ol_del = 0;
-		const int r = mab_hit2arc(h, (int)(seq[qn] & 0x7fffffffu), (int)(seq[h.tn] & 0x7fffffffu), p.max_hang, p.int_frac, p.min_ovlp, &t);
-		bool emit = false;
-		if (r >= 0) {
-			if (qn == h.tn) {
-				if ((uint32_t)h.qns == h.ts && h.qe == h.te && (h.ml_rev >> 31)) atomicOr(&seq[qn], MAB_DEL_BIT);
-			} else emit = true;
-		} else if (r == MAB_HT_QCONT) atomicOr(&seq[qn], MAB_DEL_BIT);
-		emit_flag[i] = emit;
-		cnt += emit;
-		const uint32_t prev = i ? (uint32_t)(a[i - 1].qns >> 32) : 0;
-		if (i == 0 || prev != qn) g32[2 * (size_t)qn + 1] = (uint32_t)i;
-		if (i == n - 1 || (uint32_t)(a[i + 1].qns >> 32) != qn) g32[2 * (size_t)qn] = (uint32_t)(i + 1);
-		if (i && prev > qn) bad = true;
+	unsigned m = 0;
+	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+		const uint64_t g = grp[i];
+		const unsigned c = (uint32_t)g ? (uint32_t)g - (uint32_t)(g >> 32) : 0;
+		m = c > m ? c : m;
 	}
-	cnt = __reduce_add_sync(0xffffffffu, cnt);
-	if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(scal + SC_COUNT, (unsigned long long)cnt);
-	if (bad) scal[SC_AUX2] = 1ull;
+	m = __reduce_max_sync(0xffffffffu, m);
+	if ((threadIdx.x & 31) == 0 && m) atomicMax(mx, (unsigned long long)m);
 }
 
-struct U8ToU32 { __host__ __device__ __forceinline__ uint32_t operator()(uint8_t x) const { return x; } };
-
 __global__ void __launch_bounds__(SGW_WARPS * 32)
-k_sg_sort_warp(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const uint32_t *__restrict__ epos, const uint32_t *__restrict__ seq,
-               uint32_t n_seq, HitArcParams p, uint32_t lb, DArc *__restrict__ out, uint32_t *big_list, unsigned long long *scal)
-{
+k_sg_onepass(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, uint32_t *seq, uint32_t n_seq, HitArcParams p, uint32_t lb,
+             unsigned long long *tile_ctr, ArcTileState tstate, DArc *__restrict__ out, uint64_t *__restrict__ idx, uint2 *__restrict__ big_list,
+             unsigned long long *scal)
+{	// seq: lengths are read while warps set the del bits of their own reads; lengths are masked, so this is benign
 	__shared__ uint32_t s_key[SGW_WARPS][SGW_HITS], s_v[SGW_WARPS][SGW_HITS], s_ol[SGW_WARPS][SGW_HITS];
+	__shared__ typename ArcPrefixOp::TempStorage s_pref;
+	__shared__ uint32_t s_n[SGW_WARPS], s_tile, s_base;
 	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+	const unsigned lt = (1u << lane) - 1u;
 	uint32_t *key = s_key[warp], *pv = s_v[warp], *pol = s_ol[warp];
 	const uint32_t len_mask = (1u << lb) - 1u; // lb <= 22 on this path
-	for (uint32_t r = blockIdx.x * SGW_WARPS + warp; r < n_seq; r += gridDim.x * SGW_WARPS) {
+	if (threadIdx.x == 0) s_tile = (uint32_t)atomicAdd(tile_ctr, 1ull);
+	__syncthreads();
+	const uint32_t t = s_tile, r = t * SGW_WARPS + warp;
+	uint32_t first = 0, cnt = 0, n = 0, n0 = 0; // n: arcs of this read, n0: those leaving vertex 2r (all uniform)
+	int ql = 0;
+	if (r < n_seq) {
 		const uint64_t g = grp[r];
-		const uint32_t end = (uint32_t)g, first = (uint32_t)(g >> 32);
-		if (end == 0) continue;
-		const uint32_t cnt = end - first;
-		if (cnt > SGW_HITS) { if (lane == 0) big_list[atomicAdd(scal + SC_BIG, 1ull)] = r; continue; }
-		const int ql = (int)(seq[r] & 0x7fffffffu);
-		uint32_t n = 0; // arcs of this read so far (uniform)
-		for (uint32_t c = 0; c < cnt; c += 32) {
-			bool ok = false;
-			DArc t;
-			t.ul = 0, t.v = 0, t.ol_del = 0;
-			if (c + lane < cnt) {
-				const DHit h = ld_hit(a + first + c + lane);
-				const int rr = mab_hit2arc(h, ql, (int)(seq[h.tn] & 0x7fffffffu), p.max_hang, p.int_frac, p.min_ovlp, &t);
-				ok = rr >= 0 && h.tn != r;
-			}
-			const unsigned m = __ballot_sync(0xffffffffu, ok);
-			if (ok) {
-				const uint32_t k = n + __popc(m & ((1u << lane) - 1u));
-				key[k] = ((((uint32_t)(t.ul >> 32) & 1u) << lb | (uint32_t)t.ul) << SGW_IDX_BITS) | k;
-				pv[k] = t.v, pol[k] = t.ol_del;
-			}
-			n += __popc(m);
+		if ((uint32_t)g) first = (uint32_t)(g >> 32), cnt = (uint32_t)g - first;
+		ql = (int)(seq[r] & 0x7fffffffu);
+	}
+	const bool big = cnt > SGW_HITS;
+	for (uint32_t c = 0; c < cnt; c += 32) {
+		bool ok = false;
+		DArc e;
+		e.ul = 0, e.v = 0, e.ol_del = 0;
+		if (c + lane < cnt) {
+			const DHit h = ld_hit(a + first + c + lane);
+			const int rr = mab_hit2arc(h, ql, (int)(seq[h.tn] & 0x7fffffffu), p.max_hang, p.int_frac, p.min_ovlp, &e);
+			if (rr >= 0) {
+				if (h.tn == r) { // self match: only the palindromic artefact has an effect (asm.c:27-31)
+					if ((uint32_t)h.qns == h.ts && h.qe == h.te && (h.ml_rev >> 31)) atomicOr(&seq[r], MAB_DEL_BIT);
+				} else ok = true;
+			} else if (rr == MAB_HT_QCONT) atomicOr(&seq[r], MAB_DEL_BIT);
 		}
-		if (n == 0) continue;
+		const uint32_t dir = (uint32_t)(e.ul >> 32) & 1u;
+		const unsigned m = __ballot_sync(0xffffffffu, ok), m0 = __ballot_sync(0xffffffffu, ok && dir == 0);
+		if (ok && !big) {
+			const uint32_t k = n + __popc(m & lt);
+			key[k] = ((dir << lb | (uint32_t)e.ul) << SGW_IDX_BITS) | k;
+			pv[k] = e.v, pol[k] = e.ol_del;
+		}
+		n += __popc(m), n0 += __popc(m0);
+	}
+	if (n && !big) {
 		uint32_t np = 32; while (np < n) np <<= 1;
 		__syncwarp();
 		switch (np) {
@@ -1494,47 +1504,78 @@ k_sg_sort_warp(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, con
 			default: sub_sort_regs<8>(key, n, lane); break;
 		}
 		__syncwarp();
-		const uint32_t base = epos[first];
-		for (uint32_t j = lane; j < n; j += 32) {
-			const uint32_t k = key[j], src = k & ((1u << SGW_IDX_BITS) - 1u), kl = k >> SGW_IDX_BITS;
-			*reinterpret_cast<uint4*>(out + base + j) = make_uint4(kl & len_mask, r << 1 | kl >> lb, pv[src], pol[src]);
+	}
+	if (lane == 0) {
+		s_n[warp] = n;
+		// the read's del bit is final here: the input set it, or this warp did (no other warp writes seq[r])
+		if (r < n_seq && (atomicOr(&seq[r], 0u) & MAB_DEL_BIT)) atomicAdd(scal + SC_NSEL, 1ull);
+	}
+	__syncthreads();
+	if (warp == 0) {
+		const uint32_t agg = __reduce_add_sync(0xffffffffu, lane < SGW_WARPS ? s_n[lane] : 0u);
+		if (t == 0) {
+			if (lane == 0) tstate.SetInclusive(0, agg), s_base = 0;
+		} else {
+			ArcPrefixOp op(tstate, s_pref, ::cuda::std::plus<uint32_t>(), (int)t);
+			const uint32_t ex = op(agg);
+			if (lane == 0) s_base = ex;
 		}
-		__syncwarp();
+		if (lane == 0 && agg) atomicAdd(scal + SC_COUNT, (unsigned long long)agg);
+	}
+	__syncthreads();
+	if (r >= n_seq) return;
+	uint32_t base = s_base;
+	for (int w = 0; w < warp; ++w) base += s_n[w];
+	if (lane == 0) {
+		idx[2 * (size_t)r] = n0 ? (uint64_t)base << 32 | n0 : 0;
+		idx[2 * (size_t)r + 1] = n > n0 ? (uint64_t)(base + n0) << 32 | (n - n0) : 0;
+		if (big && n) big_list[atomicAdd(scal + SC_BIG, 1ull)] = make_uint2(r, base);
+	}
+	if (big) return;
+	for (uint32_t j = lane; j < n; j += 32) {
+		const uint32_t k = key[j], src = k & ((1u << SGW_IDX_BITS) - 1u), kl = k >> SGW_IDX_BITS;
+		*reinterpret_cast<uint4*>(out + base + j) = make_uint4(kl & len_mask, r << 1 | kl >> lb, pv[src], pol[src]);
 	}
 }
 
-__global__ void __launch_bounds__(512)
-k_sg_sort_cta(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const uint32_t *__restrict__ epos, const uint32_t *__restrict__ seq,
-              const uint32_t *__restrict__ big_list, uint32_t n_big, HitArcParams p, DArc *__restrict__ out, unsigned long long *scal)
+// the reads of 257..8192 hits k_sg_onepass counted and placed: big_list[b] = (read, offset of its first arc)
+__global__ void __launch_bounds__(SGC_THREADS)
+k_sg_sort_cta(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const uint32_t *__restrict__ seq,
+              const uint2 *__restrict__ big_list, uint32_t n_big, HitArcParams p, DArc *__restrict__ out)
 {
+	typedef cub::BlockScan<uint32_t, SGC_THREADS> BS;
 	extern __shared__ __align__(16) unsigned char sg_smem[];
 	uint64_t *key = reinterpret_cast<uint64_t*>(sg_smem);         // (dir << 31 | len) << 32 | arc number
 	uint32_t *pv = reinterpret_cast<uint32_t*>(key + SGC_HITS), *pol = pv + SGC_HITS;
-	__shared__ uint32_t s_n;
+	__shared__ typename BS::TempStorage s_scan;
 	const uint32_t tid = threadIdx.x, nt = blockDim.x;
 	for (uint32_t b = blockIdx.x; b < n_big; b += gridDim.x) {
-		const uint32_t r = big_list[b];
+		const uint2 rb = big_list[b];
+		const uint32_t r = rb.x, base = rb.y;
 		const uint64_t g = grp[r];
 		const uint32_t first = (uint32_t)(g >> 32), cnt = (uint32_t)g - first;
-		if (cnt > SGC_HITS) { if (tid == 0) atomicAdd(scal + SC_AUX, 1ull); continue; }
-		if (tid == 0) s_n = 0;
-		__syncthreads();
-		const uint32_t base = epos[first];
 		const int ql = (int)(seq[r] & 0x7fffffffu);
-		for (uint32_t c = tid; c < cnt; c += nt) {
-			const DHit h = ld_hit(a + first + c);
-			DArc t;
-			t.ul = 0, t.v = 0, t.ol_del = 0;
-			const int rr = mab_hit2arc(h, ql, (int)(seq[h.tn] & 0x7fffffffu), p.max_hang, p.int_frac, p.min_ovlp, &t);
-			if (rr >= 0 && h.tn != r) {
-				const uint32_t k = epos[first + c] - base; // arcs of this read emitted before hit c
-				key[k] = (uint64_t)((((uint32_t)(t.ul >> 32) & 1u) << 31) | (uint32_t)t.ul) << 32 | k;
-				pv[k] = t.v, pol[k] = t.ol_del;
-				atomicAdd(&s_n, 1u);
+		uint32_t n = 0; // arcs of the chunks before (uniform)
+		for (uint32_t c0 = 0; c0 < cnt; c0 += nt) {
+			const uint32_t c = c0 + tid;
+			bool ok = false;
+			DArc e;
+			e.ul = 0, e.v = 0, e.ol_del = 0;
+			if (c < cnt) {
+				const DHit h = ld_hit(a + first + c);
+				const int rr = mab_hit2arc(h, ql, (int)(seq[h.tn] & 0x7fffffffu), p.max_hang, p.int_frac, p.min_ovlp, &e);
+				ok = rr >= 0 && h.tn != r;
 			}
+			uint32_t k, tot;
+			BS(s_scan).ExclusiveSum((uint32_t)ok, k, tot);
+			if (ok) {
+				k += n;
+				key[k] = (uint64_t)((((uint32_t)(e.ul >> 32) & 1u) << 31) | (uint32_t)e.ul) << 32 | k;
+				pv[k] = e.v, pol[k] = e.ol_del;
+			}
+			n += tot;
+			__syncthreads();
 		}
-		__syncthreads();
-		const uint32_t n = s_n;
 		uint32_t np = 2; while (np < n) np <<= 1;
 		for (uint32_t i = n + tid; i < np; i += nt) key[i] = ~0ull;
 		__syncthreads();
@@ -1558,52 +1599,62 @@ k_sg_sort_cta(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, cons
 	}
 }
 
-// true: g.arc holds the sorted arcs.  false: nothing usable was produced, the caller runs the column sort.
-static bool sg_emit_segmented(MabDev &d, const DHits &h, const HitArcParams &p, uint32_t lb, DGraph &g)
+// true: g.arc holds the sorted arcs, g.idx their index and *n_del the deleted reads.  false: nothing was written, the caller
+// runs the column sort.
+static bool sg_emit_segmented(MabDev &d, const DHits &h, const HitArcParams &p, uint32_t lb, DGraph &g, uint32_t *n_del)
 {
 	const size_t n = h.n;
 	const uint32_t n_seq = h.n_seq;
-	if (lb + 1 + SGW_IDX_BITS > 32 || n >= (1ull << 31)) return false;
-	uint8_t *ef = mab_alloc<uint8_t>(d, n);
-	uint32_t *epos = mab_alloc<uint32_t>(d, n), *big = mab_alloc<uint32_t>(d, n_seq);
-	uint64_t *grp = mab_alloc<uint64_t>(d, n_seq);
-	MAB_CUDA(cudaMemsetAsync(grp, 0, (size_t)n_seq * 8, d.stream));
+	if (lb + 1 + SGW_IDX_BITS > 32 || n >= (1ull << 31) || n_seq == 0) return false;
 	d.zero_scal(SC_COUNT, 5); // SC_COUNT .. SC_AUX2
-	MAB_LAUNCH(d, k_sg_classify, mab_grid(n, 256), 256, 0, h.a, n, g.seq, p, ef, (uint32_t*)grp, d.d_scal);
-	const uint32_t n_arc = (uint32_t)d.get_scal(SC_COUNT);
-	bool ok = d.h_scal[SC_AUX2] == 0; // query ids ascend
-	if (ok) {
-		cub::TransformInputIterator<uint32_t, U8ToU32, const uint8_t*> in(ef, U8ToU32());
-		size_t tb = 0;
-		cub::DeviceScan::ExclusiveSum(nullptr, tb, in, epos, (int64_t)n, d.stream);
-		void *tmp = d.tmp(tb);
-		cub::DeviceScan::ExclusiveSum(tmp, tb, in, epos, (int64_t)n, d.stream);
-		++d.n_lib;
-		dg_reserve(d, g, n_arc ? n_arc : 1);
-		unsigned grid = (n_seq + SGW_WARPS - 1) / SGW_WARPS;
-		if (grid > MAB_SMS * 32u) grid = MAB_SMS * 32u;
-		MAB_LAUNCH(d, k_sg_sort_warp, grid, SGW_WARPS * 32, 0, h.a, grp, epos, g.seq, n_seq, p, lb, g.arc, big, d.d_scal);
-		const uint32_t n_big = (uint32_t)d.get_scal(SC_BIG);
-		if (n_big) {
-				const size_t smem = (size_t)SGC_HITS * 16;
-			MAB_CUDA(cudaFuncSetAttribute(k_sg_sort_cta, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-			MAB_LAUNCH(d, k_sg_sort_cta, n_big < MAB_SMS ? n_big : MAB_SMS, 512, smem, h.a, grp, epos, g.seq, big, n_big, p, g.arc, d.d_scal);
-			if (d.get_scal(SC_AUX) != 0) ok = false; // a read with more hits than a CTA sorts
-		}
+	d.zero_scal(SC_NSEL);
+	d.zero_scal(SC_TMP0);
+	const uint64_t *grp = h.grp;
+	uint64_t *own = nullptr;
+	if (!grp) { // hits that did not come through the sort or the selection: the bounds of their runs, and whether the ids ascend
+		own = mab_alloc<uint64_t>(d, n_seq);
+		MAB_CUDA(cudaMemsetAsync(own, 0, (size_t)n_seq * 8, d.stream));
+		MAB_LAUNCH(d, k_group_bounds, mab_grid(n, 256), 256, 0, h.a, n, (uint32_t*)own, d.d_scal + SC_AUX2);
+		grp = own;
 	}
-	d.free(ef); d.free(epos); d.free(big); d.free(grp);
-	if (ok) g.len_bits = lb, g.n_arc = n_arc, g.is_srt = true, g.has_idx = false;
+	MAB_LAUNCH(d, k_grp_max, mab_grid(n_seq, 256), 256, 0, grp, n_seq, d.d_scal + SC_AUX);
+	const bool ok = d.get_scal(SC_AUX) <= (unsigned long long)SGC_HITS && d.h_scal[SC_AUX2] == 0;
+	if (ok) {
+		dg_reserve(d, g, n); // an arc never outnumbers its hits
+		const int n_tile = (int)((n_seq + SGW_WARPS - 1) / SGW_WARPS);
+		size_t ts_bytes = 0;
+		MAB_CUDA(ArcTileState::AllocationSize(n_tile, ts_bytes));
+		void *ts_mem = d.alloc(ts_bytes);
+		ArcTileState ts;
+		MAB_CUDA(ts.Init(n_tile, ts_mem, ts_bytes));
+		MAB_LAUNCH(d, k_arc_tiles_init, mab_grid((size_t)n_tile, 256, 1u << 30), 256, 0, ts, n_tile);
+		uint2 *big = mab_alloc<uint2>(d, n_seq);
+		MAB_LAUNCH(d, k_sg_onepass, n_tile, SGW_WARPS * 32, 0, h.a, grp, g.seq, n_seq, p, lb, d.d_scal + SC_TMP0, ts, g.arc, g.idx, big, d.d_scal);
+		g.n_arc = (uint32_t)d.get_scal(SC_COUNT);
+		*n_del = (uint32_t)d.h_scal[SC_NSEL];
+		const uint32_t n_big = (uint32_t)d.h_scal[SC_BIG];
+		if (n_big) {
+			const size_t smem = (size_t)SGC_HITS * 16;
+			MAB_CUDA(cudaFuncSetAttribute(k_sg_sort_cta, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+			MAB_LAUNCH(d, k_sg_sort_cta, n_big < MAB_SMS ? n_big : MAB_SMS, SGC_THREADS, smem, h.a, grp, g.seq, big, n_big, p, g.arc);
+		}
+		d.free(ts_mem); d.free(big);
+		g.len_bits = lb, g.is_srt = true, g.has_idx = true;
+	}
+	d.free(own);
 	return ok;
 }
 
 void dh_sg_gen(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g)
 {
-	dh_sg_emit(d, h, len, del, p, g);
-	dg_cleanup(d, g);
+	const int64_t n_del = dh_sg_emit(d, h, len, del, p, g);
+	// hit2arc never sets an arc's del bit: without a deleted read asg_arc_rm keeps every arc, and the sweep that finds out is skipped
+	if ((n_del < 0 ? dg_n_del_seq(d, g) : (uint32_t)n_del) != 0) dg_cleanup(d, g);
+	else if (!g.has_idx) dg_arc_index(d, g);
 	if (MAB_V(1)) fprintf(stderr, "[M::%s] read %d arcs\n", "ma_sg_gen", g.n_arc);
 }
 
-void dh_sg_emit(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g)
+int64_t dh_sg_emit(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g)
 {
 	const uint32_t n_seq = h.n_seq;
 	dg_set_nseq(d, g, n_seq);
@@ -1617,8 +1668,9 @@ void dh_sg_emit(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *d
 	if (h.n) {
 		if (h.n >= (1ull << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 arcs on one GPU\n"); exit(73); }
 		static const bool seg_sort = !(getenv("MAB_SG_SEGSORT") && atoi(getenv("MAB_SG_SEGSORT")) == 0); // default on; 0 = device-wide column sort
-		if (seg_sort && sg_emit_segmented(d, h, p, lb, g)) return;
-		if (seg_sort) d.zero_scal(SC_COUNT); // the attempt counted the arcs already
+		uint32_t n_del = 0;
+		if (seg_sort && sg_emit_segmented(d, h, p, lb, g, &n_del)) return n_del;
+		d.zero_scal(SC_COUNT);
 		const uint64_t sentinel = 1ull << (lb + bits_for((uint64_t)n_seq * 2 - 1));
 		uint64_t *ka = mab_alloc<uint64_t>(d, h.n), *kb = mab_alloc<uint64_t>(d, h.n), *va = mab_alloc<uint64_t>(d, h.n), *vb = mab_alloc<uint64_t>(d, h.n);
 		// seq lengths are read while other threads may set del bits: lengths are masked, so this is benign
@@ -1627,4 +1679,5 @@ void dh_sg_emit(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *d
 		dg_build_sorted(d, g, ka, va, kb, vb, (uint32_t)h.n, n_arc, lb, true);
 		d.free(ka); d.free(kb); d.free(va); d.free(vb);
 	} else { dg_reserve(d, g, 1); g.is_srt = true; }
+	return -1;
 }

@@ -14,8 +14,9 @@ struct DHits {
 	DHit *a = nullptr, *a2 = nullptr;   // hit array + ping-pong buffer for compaction
 	size_t n = 0, m = 0;
 	uint32_t n_seq = 0;
-	// per-read bounds of the sorted hits, first << 32 | end (0 = the read heads no hits), n_seq entries; left by the sort and
-	// dropped by every pass that moves, drops or renumbers hits (null = unknown: ma_hit_sub derives them from the hits)
+	// per-read bounds of the sorted hits, first << 32 | end (0 = the read heads no hits), n_seq entries; left by the sort and by
+	// dh_select for the renumbered reads, dropped by every other pass that moves, drops or renumbers hits (null = unknown:
+	// ma_hit_sub and ma_sg_gen derive them from the hits)
 	uint64_t *grp = nullptr;
 };
 
@@ -68,8 +69,9 @@ struct SelectHooks {
 	std::function<void(DSub*, uint8_t*, uint32_t)> flags_done;
 };
 size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t *map_out, float *cov, const SelectHooks &hk);
-// ma_sg_gen without the final asg_cleanup: seq table + sorted local arcs (sharded runs clean up after exchanging seq flags)
-void dh_sg_emit(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g);
+// ma_sg_gen without the final asg_cleanup: seq table + sorted local arcs (sharded runs clean up after exchanging seq flags).
+// Returns the number of deleted reads when the emit counted them, else -1.
+int64_t dh_sg_emit(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g);
 
 // ma_sg_gen (asm.c:9-39): lens/del per read -> graph with arcs emitted in hit order, then asg_cleanup.
 void dh_sg_gen(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g);
