@@ -355,6 +355,7 @@ int mab_select(mab_ctx_t *c, const ma_opt_t *opt, int no_first, int no_second, i
 	DHits &h = c->hits;
 	PhaseTimer pt(d, &c->stats.ms_select, "mab_select");
 	ctx_drop_graphs(c);
+	dh_hits_dense(d, h);   // a selection again: the step functions need the dense array
 	auto step3_banner = [] { if (!mab_mute && ma_verbose >= 1) fprintf(stderr, "[M::main] ===> Step 3: 2-pass (fine) read selection <===\n"); };
 	if (!no_first && !no_second && stage >= 5) { // the whole selection: per-read passes over the hit buckets
 		if (!mab_mute && ma_verbose >= 1) fprintf(stderr, "[M::main] ===> Step 2: 1-pass (crude) read selection <===\n");
@@ -535,6 +536,7 @@ ma_sub_t *mab_export_sub(mab_ctx_t *c)
 ma_hit_t *mab_export_hits(mab_ctx_t *c, size_t *n)
 {
 	MAB_CUDA(cudaSetDevice(c->dev.device));
+	dh_hits_dense(c->dev, c->hits);
 	ma_hit_t *a = (ma_hit_t*)malloc((c->hits.n ? c->hits.n : 1) * sizeof(ma_hit_t));
 	if (c->hits.n) MAB_CUDA(cudaMemcpyAsync(a, c->hits.a, c->hits.n * sizeof(DHit), cudaMemcpyDeviceToHost, c->dev.stream));
 	c->dev.sync();
@@ -603,6 +605,7 @@ long mab_write_paf(mab_ctx_t *c, FILE *fp)
 {
 	MAB_CUDA(cudaSetDevice(c->dev.device));
 	if (!c->sub) return -1;
+	dh_hits_dense(c->dev, c->hits);
 	return write_dump(c, DUMP_PAF, c->hits.n, fp);
 }
 
@@ -825,6 +828,7 @@ int mab_select_sharded(mab_ctx_t *c, const ma_opt_t *opt)
 	ShardComm &sc = c->sc;
 	PhaseTimer pt(d, &c->stats.ms_select, "mab_select_sharded");
 	ctx_drop_graphs(c);
+	dh_hits_dense(d, c->hits);
 	const int msave = mab_mute;
 	if (sc.rank != 0) mab_mute = 1; // only rank 0 talks (thread-local: ranks may be threads of one process); the counts it prints are summed over the ranks
 	mab_count_hook = sum_over_ranks, mab_count_hook_ctx = c;

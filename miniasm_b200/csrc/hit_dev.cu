@@ -44,10 +44,12 @@ __device__ __forceinline__ void st_hit(DHit *p, const DHit &h)
 static inline uint32_t bits_for(uint64_t x) { uint32_t b = 0; while (x) ++b, x >>= 1; return b ? b : 1; }
 
 static void drop_bounds(MabDev &d, DHits &h) { d.free(h.grp); h.grp = nullptr; }
+static void drop_selected(MabDev &d, DHits &h) { d.free(h.map); d.free(h.off); h.map = nullptr, h.off = nullptr; }
 
 void dh_reserve(MabDev &d, DHits &h, size_t m)
 {
 	drop_bounds(d, h);                  // the caller refills the hits
+	drop_selected(d, h);
 	if (m <= h.m) return;
 	DHit *na = mab_alloc<DHit>(d, m), *nb = mab_alloc<DHit>(d, m);
 	if (h.n) MAB_CUDA(cudaMemcpyAsync(na, h.a, h.n * sizeof(DHit), cudaMemcpyDeviceToDevice, d.stream));
@@ -58,6 +60,7 @@ void dh_reserve(MabDev &d, DHits &h, size_t m)
 void dh_free(MabDev &d, DHits &h)
 {
 	d.free(h.a); d.free(h.a2); d.free(h.grp);
+	drop_selected(d, h);
 	h = DHits();
 }
 
@@ -1089,8 +1092,9 @@ size_t dh_contained(MabDev &d, DHits &h, DSub *sub, const uint8_t *seq_del, cons
 // read's interval (the target's) and only the renumbering needs every read's containment flag; everything else is local to
 // one query read.  So the hits stay in their buckets: each pass moves a read's surviving hits to the front of its bucket
 // (in order: survivors only move down, behind everything the warp has loaded) and shrinks the bound in h.grp.  Dead slots keep
-// their read's id.  A record is stored only when it moved or its cut changed it.  One final pass renumbers the survivors
-// and writes the dense, qid-ordered array the step functions would have left.
+// their read's id.  A record is stored only when it moved or its cut changed it.  The renumbering leaves the survivors in
+// their buckets (DHits::map): ma_sg_gen reads them there, and dh_hits_dense writes the dense, qid-ordered array the step
+// functions would have left for the readers that need it.
 // ---------------------------------------------------------------------------------------------
 enum { SCS_CUT = SC_TMP0, SCS_DP, SCS_LEN, SCS_FLT, SCS_CUT2, SCS_NSEQ, SCS_NHITS }; // d_scal slots of dh_select's counters
 
@@ -1229,9 +1233,11 @@ k_sel_cut_cont(DHit *a, uint64_t *grp, uint32_t n_seq, const DSub *__restrict__ 
 	if (lane == 0 && cut) atomicAdd(n_cut, (unsigned long long)cut);
 }
 
-// hits of each kept read whose target is also kept, at the read's new id
+// hits of each kept read whose target is also kept, at the read's new id, and the read's bucket bounds in grp_out[new id] (a
+// fresh array: other warps still read grp[r] of old ids r >= m)
 __global__ void __launch_bounds__(256)
-k_sel_final_count(const uint64_t *__restrict__ grp, const uint32_t *__restrict__ tn, const int32_t *__restrict__ map, uint32_t n_seq, uint32_t *cnt)
+k_sel_final_count(const uint64_t *__restrict__ grp, const uint32_t *__restrict__ tn, const int32_t *__restrict__ map, uint32_t n_seq, uint32_t *cnt,
+                  uint64_t *__restrict__ grp_out)
 {
 	const int lane = threadIdx.x & 31;
 	for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_seq; r += (gridDim.x * blockDim.x) >> 5) {
@@ -1242,40 +1248,42 @@ k_sel_final_count(const uint64_t *__restrict__ grp, const uint32_t *__restrict__
 		unsigned c = 0;
 		if (end) for (uint32_t i = first + lane; i < end; i += 32) c += map[tn[i]] >= 0;
 		c = __reduce_add_sync(0xffffffffu, c);
-		if (lane == 0) cnt[m] = c;
+		if (lane == 0) cnt[m] = c, grp_out[m] = g;
 	}
 }
 
-// renumber the surviving hits of each kept read and write them densely at off[new id], with their bounds in grp_out[new id]
-// (a fresh array: other warps still read grp[r] of old ids r >= m); also reports the new read count (*n_new) and hit count to scal
+// A kept hit of read m (new id) read from its bucket, where it still carries the old ids: renumbered in registers.  false: its
+// target was dropped, so the dense array does not hold it.
+__device__ __forceinline__ bool sel_renumber(DHit &h, uint32_t m, const int32_t *__restrict__ map)
+{
+	const int32_t tn = map[h.tn];
+	h.qns = (uint64_t)m << 32 | (uint32_t)h.qns, h.tn = (uint32_t)tn;
+	return tn >= 0;
+}
+
+// renumber the kept hits of each kept read and write them densely at off[new id]; grp[new id] turns from the bucket bounds
+// into the dense bounds
 __global__ void __launch_bounds__(256)
-k_sel_final_copy(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const int32_t *__restrict__ map, uint32_t n_seq,
-                 const uint32_t *__restrict__ off, const uint32_t *__restrict__ n_new, DHit *__restrict__ out, uint64_t *__restrict__ grp_out,
-                 unsigned long long *scal)
+k_sel_final_copy(const DHit *__restrict__ a, uint64_t *__restrict__ grp, const int32_t *__restrict__ map, uint32_t n_seq,
+                 const uint32_t *__restrict__ off, DHit *__restrict__ out)
 {
 	const int lane = threadIdx.x & 31;
 	const unsigned lt = (1u << lane) - 1u;
-	if (blockIdx.x == 0 && threadIdx.x == 0) { const uint32_t nn = *n_new; scal[SCS_NSEQ] = nn, scal[SCS_NHITS] = off[nn]; }
-	for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_seq; r += (gridDim.x * blockDim.x) >> 5) {
-		const int32_t m = map[r];
-		if (m < 0) continue;
-		if (lane == 0) { const uint32_t s = off[m], e = off[m + 1]; grp_out[m] = e > s ? (uint64_t)s << 32 | e : 0; }
-		const uint64_t g = grp[r];
+	for (uint32_t m = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; m < n_seq; m += (gridDim.x * blockDim.x) >> 5) {
+		const uint64_t g = grp[m];
 		const uint32_t end = (uint32_t)g, first = (uint32_t)(g >> 32);
-		if (end == 0) continue;
 		uint32_t o = off[m];
-		for (uint32_t c = first; c < end; c += 32) {
+		if (end) for (uint32_t c = first; c < end; c += 32) {
 			const uint32_t i = c + lane;
 			DHit h;
-			int32_t tn = -1;
-			if (i < end) { h = ld_hit(a + i); tn = map[h.tn]; }
-			const unsigned km = __ballot_sync(0xffffffffu, tn >= 0);
-			if (tn >= 0) {
-				h.qns = (uint64_t)(uint32_t)m << 32 | (uint32_t)h.qns, h.tn = (uint32_t)tn;
-				st_hit(out + o + __popc(km & lt), h);
-			}
+			bool live = false;
+			if (i < end) { h = ld_hit(a + i); live = sel_renumber(h, m, map); }
+			const unsigned km = __ballot_sync(0xffffffffu, live);
+			if (live) st_hit(out + o + __popc(km & lt), h);
 			o += __popc(km);
 		}
+		__syncwarp(); // every lane has read grp[m]
+		if (lane == 0) { const uint32_t s = off[m]; grp[m] = o > s ? (uint64_t)s << 32 | o : 0; }
 	}
 }
 
@@ -1292,6 +1300,16 @@ static void exclusive_sum(MabDev &d, const uint32_t *in, uint32_t *out, size_t n
 	void *tmp = d.tmp(tb);
 	cub::DeviceScan::ExclusiveSum(tmp, tb, in, out, (int64_t)n, d.stream);
 	++d.n_lib;
+}
+
+void dh_hits_dense(MabDev &d, DHits &h)
+{
+	if (!h.map) return;
+	if (h.n_seq) {
+		MAB_LAUNCH(d, k_sel_final_copy, warp_grid(h.n_seq, 8), 256, 0, h.a, h.grp, h.map, h.n_seq, h.off, h.a2);
+		DHit *t = h.a; h.a = h.a2; h.a2 = t;
+	}
+	drop_selected(d, h);
 }
 
 size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t *map_out, float *cov, const SelectHooks &hk)
@@ -1337,33 +1355,37 @@ size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t 
 	dh_sub_merge(d, n_seq, sub, sub2);
 	d.trace("select:cut1+flt+sub2");
 
-	// ma_hit_cut with sub2 + ma_hit_contained's flags; h.a2 is idle until the final copy and holds the targets meanwhile
+	// ma_hit_cut with sub2 + ma_hit_contained's flags; h.a2 is idle and holds the targets meanwhile
 	uint8_t *used = mab_alloc<uint8_t>(d, n_seq);
 	uint32_t *tn = reinterpret_cast<uint32_t*>(h.a2);
 	MAB_CUDA(cudaMemsetAsync(used, 0, n_seq, d.stream));
 	MAB_LAUNCH(d, k_sel_cut_cont, warp_grid(n_seq, 8), 256, 0, h.a, h.grp, n_seq, sub2, sub, o.min_span, o.cont, used, tn, d.d_scal + SCS_CUT2);
 	if (hk.flags_done) hk.flags_done(sub, used, n_seq);
 
-	// renumbering: keep flags -> new ids (sub2 is dead and takes the compacted table), then hit counts -> offsets -> dense copy
+	// renumbering: keep flags -> new ids (sub2 is dead and takes the compacted table), then hit counts -> offsets; the kept hits
+	// stay in their buckets
 	uint32_t *keep = mab_alloc<uint32_t>(d, (size_t)n_seq + 1), *excl = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);
 	uint32_t *cnt = mab_alloc<uint32_t>(d, (size_t)n_seq + 1), *off = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);
+	int32_t *map = mab_alloc<int32_t>(d, n_seq);
+	uint64_t *grp_new = mab_alloc<uint64_t>(d, n_seq);
 	MAB_CUDA(cudaMemsetAsync(keep + n_seq, 0, 4, d.stream));
+	MAB_CUDA(cudaMemsetAsync(cnt, 0, ((size_t)n_seq + 1) * 4, d.stream));
 	MAB_LAUNCH(d, k_cont_keep, mab_grid(n_seq, 256), 256, 0, n_seq, sub, used, nullptr, keep);
 	exclusive_sum(d, keep, excl, (size_t)n_seq + 1);   // excl[n_seq] = reads kept
-	MAB_LAUNCH(d, k_cont_map, mab_grid(n_seq, 256), 256, 0, n_seq, keep, excl, map_out, sub, sub2);
-	MAB_LAUNCH(d, k_sel_final_count, warp_grid(n_seq, 8), 256, 0, h.grp, tn, map_out, n_seq, cnt); // cnt[0 ..< reads kept]
-	exclusive_sum(d, cnt, off, (size_t)n_seq + 1);      // off[reads kept] = hits kept; later entries are not used
-	uint64_t *grp_new = mab_alloc<uint64_t>(d, n_seq);
-	MAB_LAUNCH(d, k_sel_final_copy, warp_grid(n_seq, 8), 256, 0, h.a, h.grp, map_out, n_seq, off, excl + n_seq, h.a2, grp_new, d.d_scal);
+	MAB_LAUNCH(d, k_cont_map, mab_grid(n_seq, 256), 256, 0, n_seq, keep, excl, map, sub, sub2);
+	MAB_LAUNCH(d, k_sel_final_count, warp_grid(n_seq, 8), 256, 0, h.grp, tn, map, n_seq, cnt, grp_new); // cnt[0 ..< reads kept]
+	exclusive_sum(d, cnt, off, (size_t)n_seq + 1);      // off[reads kept ..= n_seq] = hits kept
+	MAB_CUDA(cudaMemcpyAsync(d.d_scal + SCS_NSEQ, excl + n_seq, 4, cudaMemcpyDeviceToDevice, d.stream)); // low halves of zeroed slots
+	MAB_CUDA(cudaMemcpyAsync(d.d_scal + SCS_NHITS, off + n_seq, 4, cudaMemcpyDeviceToDevice, d.stream));
+	if (n_seq) MAB_CUDA(cudaMemcpyAsync(map_out, map, (size_t)n_seq * 4, cudaMemcpyDeviceToDevice, d.stream));
 	const uint32_t n_new = (uint32_t)d.get_scal(SCS_NSEQ);
 	const size_t n_hits = (size_t)d.h_scal[SCS_NHITS];
 	const unsigned long long n_cut2 = d.h_scal[SCS_CUT2];
 	if (n_new) MAB_CUDA(cudaMemcpyAsync(sub, sub2, (size_t)n_new * sizeof(DSub), cudaMemcpyDeviceToDevice, d.stream));
-	d.free(sub2); d.free(used); d.free(keep); d.free(excl); d.free(cnt); d.free(off);
-	DHit *t = h.a; h.a = h.a2; h.a2 = t;
+	d.free(sub2); d.free(used); d.free(keep); d.free(excl); d.free(cnt);
 	h.n = n_hits, h.n_seq = n_new;
 	d.free(h.grp);
-	h.grp = grp_new;
+	h.grp = grp_new, h.map = map, h.off = off;
 	d.trace("select:cut2+contained");
 
 	unsigned long long gv[2] = { n_cut2, (unsigned long long)h.n };
@@ -1437,22 +1459,29 @@ typedef cub::TilePrefixCallbackOp<uint32_t, ::cuda::std::plus<uint32_t>, ArcTile
 
 __global__ void k_arc_tiles_init(ArcTileState ts, int n_tile) { ts.InitializeStatus(n_tile); }
 
-__global__ void k_grp_max(const uint64_t *grp, uint32_t n, unsigned long long *mx)
+// the most hits of one read: from the bounds, or from the dense offsets of selected hits (off != null), whose bucket bounds also
+// count the hits to dropped targets
+__global__ void k_grp_max(const uint64_t *grp, const uint32_t *off, uint32_t n, unsigned long long *mx)
 {
 	unsigned m = 0;
 	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
 		const uint64_t g = grp[i];
-		const unsigned c = (uint32_t)g ? (uint32_t)g - (uint32_t)(g >> 32) : 0;
+		const unsigned c = off ? off[i + 1] - off[i] : (uint32_t)g ? (uint32_t)g - (uint32_t)(g >> 32) : 0;
 		m = c > m ? c : m;
 	}
 	m = __reduce_max_sync(0xffffffffu, m);
 	if ((threadIdx.x & 31) == 0 && m) atomicMax(mx, (unsigned long long)m);
 }
 
+// SEL: the hits are selected, not compacted (DHits::map): grp holds bucket bounds, and a hit whose target was dropped is skipped
+// before it is classified, so that its deletion side effects do not happen either.  Arcs are numbered among the kept hits, so the
+// sort keys, and the arcs, are those of the dense array.  The warp / CTA choice goes by the bucket size; a read goes to the column
+// sort only if it keeps more than 8192 hits.
+template <bool SEL>
 __global__ void __launch_bounds__(SGW_WARPS * 32)
-k_sg_onepass(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, uint32_t *seq, uint32_t n_seq, HitArcParams p, uint32_t lb,
-             unsigned long long *tile_ctr, ArcTileState tstate, DArc *__restrict__ out, uint64_t *__restrict__ idx, uint2 *__restrict__ big_list,
-             unsigned long long *scal)
+k_sg_onepass(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const int32_t *__restrict__ map, uint32_t *seq, uint32_t n_seq,
+             HitArcParams p, uint32_t lb, unsigned long long *tile_ctr, ArcTileState tstate, DArc *__restrict__ out, uint64_t *__restrict__ idx,
+             uint2 *__restrict__ big_list, unsigned long long *scal)
 {	// seq: lengths are read while warps set the del bits of their own reads; lengths are masked, so this is benign
 	__shared__ uint32_t s_key[SGW_WARPS][SGW_HITS], s_v[SGW_WARPS][SGW_HITS], s_ol[SGW_WARPS][SGW_HITS];
 	__shared__ typename ArcPrefixOp::TempStorage s_pref;
@@ -1477,13 +1506,15 @@ k_sg_onepass(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, uint3
 		DArc e;
 		e.ul = 0, e.v = 0, e.ol_del = 0;
 		if (c + lane < cnt) {
-			const DHit h = ld_hit(a + first + c + lane);
-			const int rr = mab_hit2arc(h, ql, (int)(seq[h.tn] & 0x7fffffffu), p.max_hang, p.int_frac, p.min_ovlp, &e);
-			if (rr >= 0) {
-				if (h.tn == r) { // self match: only the palindromic artefact has an effect (asm.c:27-31)
-					if ((uint32_t)h.qns == h.ts && h.qe == h.te && (h.ml_rev >> 31)) atomicOr(&seq[r], MAB_DEL_BIT);
-				} else ok = true;
-			} else if (rr == MAB_HT_QCONT) atomicOr(&seq[r], MAB_DEL_BIT);
+			DHit h = ld_hit(a + first + c + lane);
+			if (!SEL || sel_renumber(h, r, map)) {
+				const int rr = mab_hit2arc(h, ql, (int)(seq[h.tn] & 0x7fffffffu), p.max_hang, p.int_frac, p.min_ovlp, &e);
+				if (rr >= 0) {
+					if (h.tn == r) { // self match: only the palindromic artefact has an effect (asm.c:27-31)
+						if ((uint32_t)h.qns == h.ts && h.qe == h.te && (h.ml_rev >> 31)) atomicOr(&seq[r], MAB_DEL_BIT);
+					} else ok = true;
+				} else if (rr == MAB_HT_QCONT) atomicOr(&seq[r], MAB_DEL_BIT);
+			}
 		}
 		const uint32_t dir = (uint32_t)(e.ul >> 32) & 1u;
 		const unsigned m = __ballot_sync(0xffffffffu, ok), m0 = __ballot_sync(0xffffffffu, ok && dir == 0);
@@ -1538,9 +1569,10 @@ k_sg_onepass(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, uint3
 	}
 }
 
-// the reads of 257..8192 hits k_sg_onepass counted and placed: big_list[b] = (read, offset of its first arc)
+// the reads of 257..8192 hits k_sg_onepass counted and placed: big_list[b] = (read, offset of its first arc); SEL as there
+template <bool SEL>
 __global__ void __launch_bounds__(SGC_THREADS)
-k_sg_sort_cta(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const uint32_t *__restrict__ seq,
+k_sg_sort_cta(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const int32_t *__restrict__ map, const uint32_t *__restrict__ seq,
               const uint2 *__restrict__ big_list, uint32_t n_big, HitArcParams p, DArc *__restrict__ out)
 {
 	typedef cub::BlockScan<uint32_t, SGC_THREADS> BS;
@@ -1562,9 +1594,11 @@ k_sg_sort_cta(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, cons
 			DArc e;
 			e.ul = 0, e.v = 0, e.ol_del = 0;
 			if (c < cnt) {
-				const DHit h = ld_hit(a + first + c);
-				const int rr = mab_hit2arc(h, ql, (int)(seq[h.tn] & 0x7fffffffu), p.max_hang, p.int_frac, p.min_ovlp, &e);
-				ok = rr >= 0 && h.tn != r;
+				DHit h = ld_hit(a + first + c);
+				if (!SEL || sel_renumber(h, r, map)) {
+					const int rr = mab_hit2arc(h, ql, (int)(seq[h.tn] & 0x7fffffffu), p.max_hang, p.int_frac, p.min_ovlp, &e);
+					ok = rr >= 0 && h.tn != r;
+				}
 			}
 			uint32_t k, tot;
 			BS(s_scan).ExclusiveSum((uint32_t)ok, k, tot);
@@ -1617,7 +1651,7 @@ static bool sg_emit_segmented(MabDev &d, const DHits &h, const HitArcParams &p, 
 		MAB_LAUNCH(d, k_group_bounds, mab_grid(n, 256), 256, 0, h.a, n, (uint32_t*)own, d.d_scal + SC_AUX2);
 		grp = own;
 	}
-	MAB_LAUNCH(d, k_grp_max, mab_grid(n_seq, 256), 256, 0, grp, n_seq, d.d_scal + SC_AUX);
+	MAB_LAUNCH(d, k_grp_max, mab_grid(n_seq, 256), 256, 0, grp, h.off, n_seq, d.d_scal + SC_AUX);
 	const bool ok = d.get_scal(SC_AUX) <= (unsigned long long)SGC_HITS && d.h_scal[SC_AUX2] == 0;
 	if (ok) {
 		dg_reserve(d, g, n); // an arc never outnumbers its hits
@@ -1629,14 +1663,17 @@ static bool sg_emit_segmented(MabDev &d, const DHits &h, const HitArcParams &p, 
 		MAB_CUDA(ts.Init(n_tile, ts_mem, ts_bytes));
 		MAB_LAUNCH(d, k_arc_tiles_init, mab_grid((size_t)n_tile, 256, 1u << 30), 256, 0, ts, n_tile);
 		uint2 *big = mab_alloc<uint2>(d, n_seq);
-		MAB_LAUNCH(d, k_sg_onepass, n_tile, SGW_WARPS * 32, 0, h.a, grp, g.seq, n_seq, p, lb, d.d_scal + SC_TMP0, ts, g.arc, g.idx, big, d.d_scal);
+		auto onepass = h.map ? k_sg_onepass<true> : k_sg_onepass<false>;
+		MAB_LAUNCH(d, onepass, n_tile, SGW_WARPS * 32, 0, h.a, grp, h.map, g.seq, n_seq, p, lb, d.d_scal + SC_TMP0, ts, g.arc, g.idx, big, d.d_scal);
 		g.n_arc = (uint32_t)d.get_scal(SC_COUNT);
 		*n_del = (uint32_t)d.h_scal[SC_NSEL];
 		const uint32_t n_big = (uint32_t)d.h_scal[SC_BIG];
 		if (n_big) {
 			const size_t smem = (size_t)SGC_HITS * 16;
-			MAB_CUDA(cudaFuncSetAttribute(k_sg_sort_cta, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-			MAB_LAUNCH(d, k_sg_sort_cta, n_big < MAB_SMS ? n_big : MAB_SMS, SGC_THREADS, smem, h.a, grp, g.seq, big, n_big, p, g.arc);
+			const unsigned grid = n_big < MAB_SMS ? n_big : MAB_SMS;
+			auto kern = h.map ? k_sg_sort_cta<true> : k_sg_sort_cta<false>;
+			MAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+			MAB_LAUNCH(d, kern, grid, SGC_THREADS, smem, h.a, grp, h.map, g.seq, big, n_big, p, g.arc);
 		}
 		d.free(ts_mem); d.free(big);
 		g.len_bits = lb, g.is_srt = true, g.has_idx = true;
@@ -1645,7 +1682,7 @@ static bool sg_emit_segmented(MabDev &d, const DHits &h, const HitArcParams &p, 
 	return ok;
 }
 
-void dh_sg_gen(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g)
+void dh_sg_gen(MabDev &d, DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g)
 {
 	const int64_t n_del = dh_sg_emit(d, h, len, del, p, g);
 	// hit2arc never sets an arc's del bit: without a deleted read asg_arc_rm keeps every arc, and the sweep that finds out is skipped
@@ -1654,7 +1691,7 @@ void dh_sg_gen(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *de
 	if (MAB_V(1)) fprintf(stderr, "[M::%s] read %d arcs\n", "ma_sg_gen", g.n_arc);
 }
 
-int64_t dh_sg_emit(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g)
+int64_t dh_sg_emit(MabDev &d, DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g)
 {
 	const uint32_t n_seq = h.n_seq;
 	dg_set_nseq(d, g, n_seq);
@@ -1670,6 +1707,7 @@ int64_t dh_sg_emit(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t
 		static const bool seg_sort = !(getenv("MAB_SG_SEGSORT") && atoi(getenv("MAB_SG_SEGSORT")) == 0); // default on; 0 = device-wide column sort
 		uint32_t n_del = 0;
 		if (seg_sort && sg_emit_segmented(d, h, p, lb, g, &n_del)) return n_del;
+		dh_hits_dense(d, h);
 		d.zero_scal(SC_COUNT);
 		const uint64_t sentinel = 1ull << (lb + bits_for((uint64_t)n_seq * 2 - 1));
 		uint64_t *ka = mab_alloc<uint64_t>(d, h.n), *kb = mab_alloc<uint64_t>(d, h.n), *va = mab_alloc<uint64_t>(d, h.n), *vb = mab_alloc<uint64_t>(d, h.n);

@@ -18,6 +18,12 @@ struct DHits {
 	// dh_select for the renumbered reads, dropped by every other pass that moves, drops or renumbers hits (null = unknown:
 	// ma_hit_sub and ma_sg_gen derive them from the hits)
 	uint64_t *grp = nullptr;
+	// Selected, not compacted (left by dh_select; null = the hits are dense): the n kept hits still lie in their read's buckets
+	// of a, under the old read ids, and grp[new id] holds those bucket bounds, which also cover the read's hits to dropped
+	// targets.  map[old id] = new id or -1; off[new id] = where the read's kept hits start in the dense order (n_seq + 1 entries).
+	// ma_sg_gen reads the buckets through map; every other reader calls dh_hits_dense first.
+	int32_t *map = nullptr;
+	uint32_t *off = nullptr;
 };
 
 struct HitArcParams { int max_hang; float int_frac; int min_ovlp; };
@@ -58,7 +64,7 @@ size_t dh_contained(MabDev &d, DHits &h, DSub *sub, const uint8_t *seq_del, cons
 // ma_sub_merge, ma_hit_cut and ma_hit_contained, with the same results and [M::...] lines as calling the steps above in turn.
 // Runs as per-read passes over the hits' per-read buckets (h.grp; derived from the hits when null).  sub: n_seq entries, the
 // merged table compacted like dh_contained's.  Returns the new hit count; h.n_seq is the surviving read count and
-// map_out[old] = new id or -1.
+// map_out[old] = new id or -1.  The hits are left selected, not compacted (see DHits::map).
 struct SelectParams { int min_dp; float min_iden; int min_span; int flt_max_hang, flt_min_ovlp; HitArcParams cont; };
 // Callbacks of dh_select; an empty member is skipped.  step3: where the second round begins (after the ma_hit_flt line).
 // sub_done(table): after each ma_hit_sub, with the n_seq rows it wrote.  flags_done(sub, used, n_seq): after the containment
@@ -69,9 +75,13 @@ struct SelectHooks {
 	std::function<void(DSub*, uint8_t*, uint32_t)> flags_done;
 };
 size_t dh_select(MabDev &d, DHits &h, DSub *sub, const SelectParams &o, int32_t *map_out, float *cov, const SelectHooks &hk);
+// The hits as the dense, qid-ordered array the step functions leave: copies the kept hits of a selection out of their buckets
+// and renumbers them (nothing to do when they are dense already).
+void dh_hits_dense(MabDev &d, DHits &h);
 // ma_sg_gen without the final asg_cleanup: seq table + sorted local arcs (sharded runs clean up after exchanging seq flags).
-// Returns the number of deleted reads when the emit counted them, else -1.
-int64_t dh_sg_emit(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g);
+// Returns the number of deleted reads when the emit counted them, else -1.  Selected hits stay in their buckets unless the
+// column sort has to take them.
+int64_t dh_sg_emit(MabDev &d, DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g);
 
 // ma_sg_gen (asm.c:9-39): lens/del per read -> graph with arcs emitted in hit order, then asg_cleanup.
-void dh_sg_gen(MabDev &d, const DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g);
+void dh_sg_gen(MabDev &d, DHits &h, const uint32_t *len, const uint8_t *del, const HitArcParams &p, DGraph &g);
