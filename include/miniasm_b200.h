@@ -159,9 +159,17 @@ void mab_set_verbose(int level);                        /* 0 silences the [M::..
 const mab_stats_t *mab_stats(const mab_ctx_t *ctx);
 
 /* Step 1, main.c:117-118 / hit.c:70-107.  The PAF bytes go to HBM once (from a host buffer, or from a plain/gzip
- * file through pinned staging buffers); parsing, the name dictionary, mirrored hits and ma_hit_sort run there. */
+ * file through pinned staging buffers); parsing, the name dictionary, mirrored hits and ma_hit_sort run there.
+ * mab_load_paf_file: a regular file that starts with the gzip magic crosses PCIe compressed and is inflated on the GPU
+ * (single or concatenated members, CRC-32 and ISIZE checked); a stream the GPU decoder rejects (damaged, trailing bytes, ...)
+ * and stdin ("-") go through zlib's gzread on the host, so the loaded bytes are the same either way. */
 int mab_load_paf_text(mab_ctx_t *ctx, const char *text, size_t len);
 int mab_load_paf_file(mab_ctx_t *ctx, const char *fn);  /* -1 if the file cannot be opened */
+/* gzip-compressed PAF held in host memory, inflated on the GPU.  Returns 0, or -2 when the GPU decoder rejects the stream:
+ * then nothing is loaded (the text is empty) and the caller inflates on the host and uses mab_load_paf_text. */
+int mab_load_paf_gz(mab_ctx_t *ctx, const void *gz, size_t len);
+/* Copies min(cap, length) bytes of the resident PAF text to dst; returns its length. */
+size_t mab_paf_text(const mab_ctx_t *ctx, char *dst, size_t cap);
 int mab_ingest(mab_ctx_t *ctx, int min_span, int min_match, int bi_dir);
 /* load + ingest overlapped: chunks of the host text are parsed while the next ones cross PCIe (same result as the two calls) */
 int mab_load_ingest_text(mab_ctx_t *ctx, const char *text, size_t len, int min_span, int min_match, int bi_dir);
@@ -196,7 +204,8 @@ long mab_write_bed(mab_ctx_t *ctx, FILE *fp); /* print_subs of main.c:13-19; -1 
 long mab_write_sg(mab_ctx_t *ctx, FILE *fp);  /* ma_sg_print(mab_export_sg, mab_export_dict, mab_export_sub); -1 before mab_layout */
 /* -f reads: ma_ug_seq (asm.c:236-290) + ma_ug_print on the GPU.  mab_reads_prefetch starts streaming the FASTA/FASTQ file (plain
  * or gzip, "-" = stdin) into HBM on a thread and stream of its own -- call it before mab_ingest and the copy hides behind the
- * graph stages.  mab_write_gfa_reads indexes the records in HBM (line starts, headers, a name table of the layout's reads),
+ * graph stages; a regular gzip file crosses PCIe compressed and is inflated on the GPU, with zlib's gzread as the fallback for
+ * a stream the GPU decoder rejects, as in mab_load_paf_file.  mab_write_gfa_reads indexes the records in HBM (line starts, headers, a name table of the layout's reads),
  * gathers / reverse-complements the bases straight into the S lines of the GFA text and writes it.  Returns the bytes written;
  * -1 before mab_unitigs; -2 (nothing written) when the file is neither FASTA-like nor 4-line FASTQ -- multi-line FASTQ cannot be
  * cut into records in parallel -- in which case the caller uses mab_export_* + ma_ug_seq + ma_ug_print. */

@@ -138,6 +138,8 @@ _PRODUCT_ONLY = {
     "mab_stats": (C.POINTER(MabStats), [C.c_void_p]),
     "mab_load_paf_text": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "mab_load_paf_file": (C.c_int, [C.c_void_p, C.c_char_p]),
+    "mab_load_paf_gz": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "mab_paf_text": (C.c_size_t, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "mab_ingest": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int]),
     "mab_load_ingest_text": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int]),
     "mab_ingest_nocont": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),

@@ -11,6 +11,7 @@
 #include <pthread.h>
 #include "ingest_dev.cuh"
 #include "shard_comm.cuh"
+#include "gunzip_dev.cuh"
 #include <cub/cub.cuh>
 #include <map>
 #include <string>
@@ -201,20 +202,145 @@ int mab_load_paf_text(mab_ctx_t *c, const char *text, size_t len)
 	return 0;
 }
 
+/* ---- gzip input inflated on the GPU (gunzip_dev.cu) ------------------------------------------------------------------ */
+struct ArenaMem : GzMem { // the PAF path's scratch: the context's arena (same stream, so frees are immediate)
+	MabDev &d;
+	explicit ArenaMem(MabDev &dev) : d(dev) {}
+	void *alloc(size_t b) override { return d.alloc(b); }
+	void free(void *p) override { d.free(p); }
+};
+
+struct PlainMem : GzMem { // the reads loader's scratch: cudaMalloc on its own thread
+	void *alloc(size_t b) override { void *p; MAB_CUDA(cudaMalloc(&p, b)); return p; }
+	void free(void *p) override { MAB_CUDA(cudaFree(p)); }
+};
+
+static void gz_trace(const char *what, const GzStats &s, double ms_raw, int rc)
+{
+	if (!getenv("MAB_TRACE")) return;
+	fprintf(stderr, "[T::gunzip] %s rc %d: raw+h2d %.3f find %.3f decode %.3f chain %.3f window %.3f resolve %.3f crc %.3f ms; "
+	        "%lu chunks, %lu units, %lu chained, %lu confirmed, %lu members, %lu bytes out, scratch peak %lu\n", what, rc, ms_raw,
+	        s.ms_find, s.ms_decode, s.ms_chain, s.ms_window, s.ms_resolve, s.ms_crc, (unsigned long)s.n_chunks, (unsigned long)s.n_units,
+	        (unsigned long)s.n_chain, (unsigned long)s.n_confirmed, (unsigned long)s.n_members, (unsigned long)s.out_len, (unsigned long)s.scratch_peak);
+}
+
+// the regular file fn when it starts with the gzip magic: an open descriptor and its size; -1 otherwise
+static int gz_open_regular(const char *fn, size_t *size)
+{
+	if (!fn || !strcmp(fn, "-")) return -1;
+	const int fd = open(fn, O_RDONLY);
+	if (fd < 0) return -1;
+	struct stat sb;
+	uint8_t mg[2];
+	if (fstat(fd, &sb) == 0 && S_ISREG(sb.st_mode) && pread(fd, mg, 2, 0) == 2 && gz_magic(mg, 2)) { *size = (size_t)sb.st_size; return fd; }
+	close(fd);
+	return -1;
+}
+
+// size bytes of fd to dst (device) through two pinned staging buffers of CH bytes: the read of chunk k+1 overlaps the copy of chunk k
+static bool read_to_dev(int fd, size_t size, char *dst, char *const pin[2], size_t CH, cudaStream_t st)
+{
+	cudaEvent_t ev[2];
+	for (int i = 0; i < 2; ++i) MAB_CUDA(cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming));
+	size_t done = 0;
+	bool ok = true;
+	for (int k = 0; ok && done < size; k ^= 1) {
+		MAB_CUDA(cudaEventSynchronize(ev[k]));
+		const size_t want = size - done < CH ? size - done : CH;
+		size_t got = 0;
+		while (got < want) {
+			const ssize_t r = pread(fd, pin[k] + got, want - got, (off_t)(done + got));
+			if (r <= 0) { ok = false; break; }
+			got += (size_t)r;
+		}
+		if (!ok) break;
+		MAB_CUDA(cudaMemcpyAsync(dst + done, pin[k], got, cudaMemcpyHostToDevice, st));
+		MAB_CUDA(cudaEventRecord(ev[k], st));
+		done += got;
+	}
+	MAB_CUDA(cudaStreamSynchronize(st));
+	for (int i = 0; i < 2; ++i) MAB_CUDA(cudaEventDestroy(ev[i]));
+	return ok;
+}
+
+static void pins_reserve(mab_ctx *c, size_t CH)
+{
+	if (c->pin_bytes >= CH) return;
+	for (int i = 0; i < 2; ++i) { if (c->pin[i]) MAB_CUDA(cudaFreeHost(c->pin[i])); MAB_CUDA(cudaMallocHost(&c->pin[i], CH)); }
+	c->pin_bytes = CH;
+}
+
+static char *paf_out(void *p, size_t n) // the inflated PAF lands in the context's text buffer
+{
+	mab_ctx *c = (mab_ctx*)p;
+	text_reserve(c, n);
+	return c->d_text;
+}
+
+// gz[0, len) in device memory (scratch of the arena) -> the context's text; GZ_OK or GZ_REJECT (then the text is empty)
+static int paf_inflate(mab_ctx *c, const char *d_gz, size_t len, const char *what, double ms_raw)
+{
+	ArenaMem am(c->dev);
+	GzStats gs;
+	memset(&gs, 0, sizeof(gs));
+	size_t n = 0;
+	const int rc = gz_inflate_dev(c->dev.stream, am, (const uint8_t*)d_gz, len, paf_out, c, &n, &gs);
+	c->text_len = rc == GZ_OK ? n : 0;
+	if (rc == GZ_OK && c->text_cap > n) MAB_CUDA(cudaMemsetAsync(c->d_text + n, 0, c->text_cap - n, c->dev.stream)); // text_reserve's rule
+	c->dev.sync();
+	gz_trace(what, gs, ms_raw, rc);
+	return rc;
+}
+
+/* gzip PAF in host memory, inflated on the GPU: 0, or -2 (nothing loaded) when the GPU decoder rejects the stream */
+int mab_load_paf_gz(mab_ctx_t *c, const void *gz, size_t len)
+{
+	MAB_CUDA(cudaSetDevice(c->dev.device));
+	ctx_reset_reads(c);
+	c->text_len = 0;
+	if (!gz_magic(gz, len)) return -2;
+	const double t0 = sys_realtime();
+	char *d_gz = (char*)c->dev.alloc(len);
+	MAB_CUDA(cudaMemcpyAsync(d_gz, gz, len, cudaMemcpyHostToDevice, c->dev.stream));
+	c->dev.sync();
+	const int rc = paf_inflate(c, d_gz, len, "mab_load_paf_gz", (sys_realtime() - t0) * 1e3);
+	c->dev.free(d_gz);
+	return rc == GZ_OK ? 0 : -2;
+}
+
+size_t mab_paf_text(const mab_ctx_t *c, char *dst, size_t cap)
+{
+	MAB_CUDA(cudaSetDevice(c->dev.device));
+	const size_t n = c->text_len < cap ? c->text_len : cap;
+	if (n) MAB_CUDA(cudaMemcpy(dst, c->d_text, n, cudaMemcpyDeviceToHost));
+	return c->text_len;
+}
+
 /* PAF file (plain or gzip, "-" = stdin) to the GPU through two pinned staging buffers: the read of chunk
- * k+1 overlaps the H2D copy of chunk k.  Returns 0, or -1 if the file cannot be opened. */
+ * k+1 overlaps the H2D copy of chunk k.  A regular gzip file crosses compressed and is inflated on the GPU; what the
+ * GPU decoder rejects goes through gzread like plain files and stdin.  Returns 0, or -1 if the file cannot be opened. */
 int mab_load_paf_file(mab_ctx_t *c, const char *fn)
 {
 	MAB_CUDA(cudaSetDevice(c->dev.device));
 	const size_t CH = 64u << 20;
+	size_t gz_size = 0;
+	const int gz_fd = gz_open_regular(fn, &gz_size);
+	if (gz_fd >= 0) {
+		ctx_reset_reads(c);
+		pins_reserve(c, CH);
+		const double t0 = sys_realtime();
+		char *d_gz = (char*)c->dev.alloc(gz_size);
+		int rc = GZ_REJECT;
+		if (read_to_dev(gz_fd, gz_size, d_gz, c->pin, CH, c->dev.stream)) rc = paf_inflate(c, d_gz, gz_size, "mab_load_paf_file", (sys_realtime() - t0) * 1e3);
+		c->dev.free(d_gz);
+		close(gz_fd);
+		if (rc == GZ_OK) return 0;
+	}
 	gzFile fp = fn && strcmp(fn, "-") ? gzopen(fn, "r") : gzdopen(fileno(stdin), "r");
 	if (fp == 0) return -1;
 	gzbuffer(fp, 1 << 20);
 	ctx_reset_reads(c);
-	if (c->pin_bytes < CH) {
-		for (int i = 0; i < 2; ++i) { if (c->pin[i]) MAB_CUDA(cudaFreeHost(c->pin[i])); MAB_CUDA(cudaMallocHost(&c->pin[i], CH)); }
-		c->pin_bytes = CH;
-	}
+	pins_reserve(c, CH);
 	struct stat sb;
 	size_t guess = 0;
 	if (fn && strcmp(fn, "-") && stat(fn, &sb) == 0) guess = (size_t)sb.st_size;
@@ -626,6 +752,42 @@ long mab_write_sg(mab_ctx_t *c, FILE *fp)
 }
 
 /* ---- -f reads (ma_ug_seq, asm.c:236-290) ------------------------------------------------------------------------------- */
+static char *reads_out(void *p, size_t n) // the inflated reads land in a buffer of the loader's own
+{
+	mab_ctx::ReadsLoad *rl = (mab_ctx::ReadsLoad*)p;
+	rl->cap = n + 4096;
+	MAB_CUDA(cudaMalloc(&rl->d_text, rl->cap));
+	return rl->d_text;
+}
+
+// a regular gzip reads file: compressed bytes to HBM, inflated there; false (nothing kept) when the GPU decoder rejects it
+static bool reads_gunzip(mab_ctx::ReadsLoad *rl, int fd, size_t size, size_t CH)
+{
+	cudaStream_t st;
+	char *pin[2], *d_gz;
+	MAB_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+	for (int i = 0; i < 2; ++i) MAB_CUDA(cudaMallocHost(&pin[i], CH));
+	MAB_CUDA(cudaMalloc(&d_gz, size));
+	const double t0 = sys_realtime();
+	int rc = GZ_REJECT;
+	GzStats gs;
+	memset(&gs, 0, sizeof(gs));
+	if (read_to_dev(fd, size, d_gz, pin, CH, st)) {
+		const double ms_raw = (sys_realtime() - t0) * 1e3;
+		PlainMem pm;
+		size_t n = 0;
+		rc = gz_inflate_dev(st, pm, (const uint8_t*)d_gz, size, reads_out, rl, &n, &gs);
+		if (rc == GZ_OK) { rl->len = n; MAB_CUDA(cudaMemsetAsync(rl->d_text + n, 0, rl->cap - n, st)); }
+		MAB_CUDA(cudaStreamSynchronize(st));
+		gz_trace("reads_loader", gs, ms_raw, rc);
+	}
+	if (rc != GZ_OK && rl->d_text) { MAB_CUDA(cudaFree(rl->d_text)); rl->d_text = nullptr, rl->len = rl->cap = 0; }
+	MAB_CUDA(cudaFree(d_gz));
+	for (int i = 0; i < 2; ++i) MAB_CUDA(cudaFreeHost(pin[i]));
+	MAB_CUDA(cudaStreamDestroy(st));
+	return rc == GZ_OK;
+}
+
 static void *reads_loader(void *p) // file -> pinned double buffer -> HBM, on a stream of its own
 {
 	mab_ctx::ReadsLoad *rl = (mab_ctx::ReadsLoad*)p;
@@ -634,6 +796,13 @@ static void *reads_loader(void *p) // file -> pinned double buffer -> HBM, on a 
 	char *pin[2];
 	cudaEvent_t ev[2];
 	MAB_CUDA(cudaSetDevice(rl->device));
+	size_t gz_size = 0;
+	const int gz_fd = gz_open_regular(rl->fn.c_str(), &gz_size);
+	if (gz_fd >= 0) {
+		const bool ok = reads_gunzip(rl, gz_fd, gz_size, CH);
+		close(gz_fd);
+		if (ok) return 0;
+	}
 	gzFile fp = rl->fn != "-" ? gzopen(rl->fn.c_str(), "r") : gzdopen(fileno(stdin), "r");
 	if (fp == 0) { rl->rc = -1; return 0; }
 	gzbuffer(fp, 1 << 20);
