@@ -1413,8 +1413,11 @@ __global__ void k_seq_set(uint32_t n_seq, const uint32_t *len, const uint8_t *de
 }
 
 // one (key, value) column pair per hit: key = u << lb | len (or the sentinel 1 << (lb + vertex bits) when the hit yields no arc),
-// value = ol:del << 32 | v.  Sorting the columns (stable) and dropping the sentinels equals asg.c's append + sort.
-__global__ void k_sg_arcs(const DHit *a, size_t n, uint32_t *seq, HitArcParams p, uint32_t lb, uint64_t sentinel, uint64_t *key, uint64_t *val, unsigned long long *n_emit)
+// value = ol:del << 32 | v.  Sorting the columns (stable) and dropping the sentinels equals asg.c's append + sort.  len32: the
+// 32-bit read lengths ma_hit2arc takes (asm.c:23-24).  An arc of 2^lb or more raises *ovf; the caller then redoes the columns
+// with lb = 32.
+__global__ void k_sg_arcs(const DHit *a, size_t n, const uint32_t *len32, uint32_t *seq, HitArcParams p, uint32_t lb, uint64_t sentinel, uint64_t *key, uint64_t *val,
+                          unsigned long long *n_emit, unsigned long long *ovf)
 {
 	unsigned cnt = 0;
 	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -1422,13 +1425,14 @@ __global__ void k_sg_arcs(const DHit *a, size_t n, uint32_t *seq, HitArcParams p
 		const uint32_t qn = (uint32_t)(h.qns >> 32);
 		DArc t;
 		t.ul = 0, t.v = 0, t.ol_del = 0;
-		int r = mab_hit2arc(h, (int)(seq[qn] & 0x7fffffffu), (int)(seq[h.tn] & 0x7fffffffu), p.max_hang, p.int_frac, p.min_ovlp, &t);
+		int r = mab_hit2arc(h, (int)len32[qn], (int)len32[h.tn], p.max_hang, p.int_frac, p.min_ovlp, &t);
 		bool emit = false;
 		if (r >= 0) {
 			if (qn == h.tn) { // self match: only the palindromic artefact has an effect (asm.c:27-31)
 				if ((uint32_t)h.qns == h.ts && h.qe == h.te && (h.ml_rev >> 31)) atomicOr(&seq[qn], MAB_DEL_BIT);
 			} else emit = true;
 		} else if (r == MAB_HT_QCONT) atomicOr(&seq[qn], MAB_DEL_BIT);
+		if (emit && lb < 32 && (uint32_t)t.ul >> lb) *ovf = 1;
 		key[i] = emit ? ((t.ul >> 32) << lb | (uint32_t)t.ul) : sentinel;
 		val[i] = (uint64_t)t.ol_del << 32 | t.v;
 		cnt += emit;
@@ -1479,10 +1483,11 @@ __global__ void k_grp_max(const uint64_t *grp, const uint32_t *off, uint32_t n, 
 // sort only if it keeps more than 8192 hits.
 template <bool SEL>
 __global__ void __launch_bounds__(SGW_WARPS * 32)
-k_sg_onepass(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const int32_t *__restrict__ map, uint32_t *seq, uint32_t n_seq,
-             HitArcParams p, uint32_t lb, unsigned long long *tile_ctr, ArcTileState tstate, DArc *__restrict__ out, uint64_t *__restrict__ idx,
-             uint2 *__restrict__ big_list, unsigned long long *scal)
-{	// seq: lengths are read while warps set the del bits of their own reads; lengths are masked, so this is benign
+k_sg_onepass(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const int32_t *__restrict__ map, const uint32_t *__restrict__ len32,
+             uint32_t *seq, uint32_t n_seq, HitArcParams p, uint32_t lb, unsigned long long *tile_ctr, ArcTileState tstate, DArc *__restrict__ out,
+             uint64_t *__restrict__ idx, uint2 *__restrict__ big_list, unsigned long long *scal)
+{	// len32: the 32-bit read lengths ma_hit2arc takes (asm.c:23-24); seq only gets del bits.  An arc of 2^lb or more (a hit that
+	// lies past its read's end) raises scal[SC_TMP0 + 1]; the caller then discards this pass and runs the column sort.
 	__shared__ uint32_t s_key[SGW_WARPS][SGW_HITS], s_v[SGW_WARPS][SGW_HITS], s_ol[SGW_WARPS][SGW_HITS];
 	__shared__ typename ArcPrefixOp::TempStorage s_pref;
 	__shared__ uint32_t s_n[SGW_WARPS], s_tile, s_base;
@@ -1498,7 +1503,7 @@ k_sg_onepass(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const
 	if (r < n_seq) {
 		const uint64_t g = grp[r];
 		if ((uint32_t)g) first = (uint32_t)(g >> 32), cnt = (uint32_t)g - first;
-		ql = (int)(seq[r] & 0x7fffffffu);
+		ql = (int)len32[r];
 	}
 	const bool big = cnt > SGW_HITS;
 	for (uint32_t c = 0; c < cnt; c += 32) {
@@ -1508,7 +1513,7 @@ k_sg_onepass(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const
 		if (c + lane < cnt) {
 			DHit h = ld_hit(a + first + c + lane);
 			if (!SEL || sel_renumber(h, r, map)) {
-				const int rr = mab_hit2arc(h, ql, (int)(seq[h.tn] & 0x7fffffffu), p.max_hang, p.int_frac, p.min_ovlp, &e);
+				const int rr = mab_hit2arc(h, ql, (int)len32[h.tn], p.max_hang, p.int_frac, p.min_ovlp, &e);
 				if (rr >= 0) {
 					if (h.tn == r) { // self match: only the palindromic artefact has an effect (asm.c:27-31)
 						if ((uint32_t)h.qns == h.ts && h.qe == h.te && (h.ml_rev >> 31)) atomicOr(&seq[r], MAB_DEL_BIT);
@@ -1517,6 +1522,7 @@ k_sg_onepass(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const
 			}
 		}
 		const uint32_t dir = (uint32_t)(e.ul >> 32) & 1u;
+		if (ok && (uint32_t)e.ul > len_mask) scal[SC_TMP0 + 1] = 1; // (big reads too: the CTA pass sorts the same arcs)
 		const unsigned m = __ballot_sync(0xffffffffu, ok), m0 = __ballot_sync(0xffffffffu, ok && dir == 0);
 		if (ok && !big) {
 			const uint32_t k = n + __popc(m & lt);
@@ -1572,7 +1578,7 @@ k_sg_onepass(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const
 // the reads of 257..8192 hits k_sg_onepass counted and placed: big_list[b] = (read, offset of its first arc); SEL as there
 template <bool SEL>
 __global__ void __launch_bounds__(SGC_THREADS)
-k_sg_sort_cta(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const int32_t *__restrict__ map, const uint32_t *__restrict__ seq,
+k_sg_sort_cta(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, const int32_t *__restrict__ map, const uint32_t *__restrict__ len32,
               const uint2 *__restrict__ big_list, uint32_t n_big, HitArcParams p, DArc *__restrict__ out)
 {
 	typedef cub::BlockScan<uint32_t, SGC_THREADS> BS;
@@ -1586,7 +1592,7 @@ k_sg_sort_cta(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, cons
 		const uint32_t r = rb.x, base = rb.y;
 		const uint64_t g = grp[r];
 		const uint32_t first = (uint32_t)(g >> 32), cnt = (uint32_t)g - first;
-		const int ql = (int)(seq[r] & 0x7fffffffu);
+		const int ql = (int)len32[r];
 		uint32_t n = 0; // arcs of the chunks before (uniform)
 		for (uint32_t c0 = 0; c0 < cnt; c0 += nt) {
 			const uint32_t c = c0 + tid;
@@ -1596,7 +1602,7 @@ k_sg_sort_cta(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, cons
 			if (c < cnt) {
 				DHit h = ld_hit(a + first + c);
 				if (!SEL || sel_renumber(h, r, map)) {
-					const int rr = mab_hit2arc(h, ql, (int)(seq[h.tn] & 0x7fffffffu), p.max_hang, p.int_frac, p.min_ovlp, &e);
+					const int rr = mab_hit2arc(h, ql, (int)len32[h.tn], p.max_hang, p.int_frac, p.min_ovlp, &e);
 					ok = rr >= 0 && h.tn != r;
 				}
 			}
@@ -1633,16 +1639,16 @@ k_sg_sort_cta(const DHit *__restrict__ a, const uint64_t *__restrict__ grp, cons
 	}
 }
 
-// true: g.arc holds the sorted arcs, g.idx their index and *n_del the deleted reads.  false: nothing was written, the caller
-// runs the column sort.
-static bool sg_emit_segmented(MabDev &d, const DHits &h, const HitArcParams &p, uint32_t lb, DGraph &g, uint32_t *n_del)
+// true: g.arc holds the sorted arcs, g.idx their index and *n_del the deleted reads.  false: the caller runs the column sort, which
+// rewrites g.arc and g.idx (if an arc outgrew lb, the del bits set in g.seq here are ones the column sort sets too).
+static bool sg_emit_segmented(MabDev &d, const DHits &h, const uint32_t *len32, const HitArcParams &p, uint32_t lb, DGraph &g, uint32_t *n_del)
 {
 	const size_t n = h.n;
 	const uint32_t n_seq = h.n_seq;
 	if (lb + 1 + SGW_IDX_BITS > 32 || n >= (1ull << 31) || n_seq == 0) return false;
 	d.zero_scal(SC_COUNT, 5); // SC_COUNT .. SC_AUX2
 	d.zero_scal(SC_NSEL);
-	d.zero_scal(SC_TMP0);
+	d.zero_scal(SC_TMP0, 2);
 	const uint64_t *grp = h.grp;
 	uint64_t *own = nullptr;
 	if (!grp) { // hits that did not come through the sort or the selection: the bounds of their runs, and whether the ids ascend
@@ -1652,7 +1658,7 @@ static bool sg_emit_segmented(MabDev &d, const DHits &h, const HitArcParams &p, 
 		grp = own;
 	}
 	MAB_LAUNCH(d, k_grp_max, mab_grid(n_seq, 256), 256, 0, grp, h.off, n_seq, d.d_scal + SC_AUX);
-	const bool ok = d.get_scal(SC_AUX) <= (unsigned long long)SGC_HITS && d.h_scal[SC_AUX2] == 0;
+	bool ok = d.get_scal(SC_AUX) <= (unsigned long long)SGC_HITS && d.h_scal[SC_AUX2] == 0;
 	if (ok) {
 		dg_reserve(d, g, n); // an arc never outnumbers its hits
 		const int n_tile = (int)((n_seq + SGW_WARPS - 1) / SGW_WARPS);
@@ -1664,19 +1670,20 @@ static bool sg_emit_segmented(MabDev &d, const DHits &h, const HitArcParams &p, 
 		MAB_LAUNCH(d, k_arc_tiles_init, mab_grid((size_t)n_tile, 256, 1u << 30), 256, 0, ts, n_tile);
 		uint2 *big = mab_alloc<uint2>(d, n_seq);
 		auto onepass = h.map ? k_sg_onepass<true> : k_sg_onepass<false>;
-		MAB_LAUNCH(d, onepass, n_tile, SGW_WARPS * 32, 0, h.a, grp, h.map, g.seq, n_seq, p, lb, d.d_scal + SC_TMP0, ts, g.arc, g.idx, big, d.d_scal);
+		MAB_LAUNCH(d, onepass, n_tile, SGW_WARPS * 32, 0, h.a, grp, h.map, len32, g.seq, n_seq, p, lb, d.d_scal + SC_TMP0, ts, g.arc, g.idx, big, d.d_scal);
 		g.n_arc = (uint32_t)d.get_scal(SC_COUNT);
 		*n_del = (uint32_t)d.h_scal[SC_NSEL];
 		const uint32_t n_big = (uint32_t)d.h_scal[SC_BIG];
-		if (n_big) {
+		ok = d.h_scal[SC_TMP0 + 1] == 0; // else an arc outgrew lb: the column sort redoes it all (the del bits set here are its own too)
+		if (ok && n_big) {
 			const size_t smem = (size_t)SGC_HITS * 16;
 			const unsigned grid = n_big < MAB_SMS ? n_big : MAB_SMS;
 			auto kern = h.map ? k_sg_sort_cta<true> : k_sg_sort_cta<false>;
 			MAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-			MAB_LAUNCH(d, kern, grid, SGC_THREADS, smem, h.a, grp, h.map, g.seq, big, n_big, p, g.arc);
+			MAB_LAUNCH(d, kern, grid, SGC_THREADS, smem, h.a, grp, h.map, len32, big, n_big, p, g.arc);
 		}
 		d.free(ts_mem); d.free(big);
-		g.len_bits = lb, g.is_srt = true, g.has_idx = true;
+		if (ok) g.len_bits = lb, g.is_srt = true, g.has_idx = true;
 	}
 	d.free(own);
 	return ok;
@@ -1700,20 +1707,25 @@ int64_t dh_sg_emit(MabDev &d, DHits &h, const uint32_t *len, const uint8_t *del,
 	d.zero_scal(SC_COUNT);
 	unsigned *d_max = (unsigned*)(d.d_scal + SC_AUX);
 	if (n_seq) MAB_LAUNCH(d, k_seq_set, mab_grid(n_seq, 256), 256, 0, n_seq, len, del, g.seq, d_max);
-	const unsigned mx = (unsigned)(d.get_scal(SC_AUX) & 0xffffffffu); // an arc is never longer than its source read (miniasm.h:97-98)
-	const uint32_t lb = bits_for(mx);
+	const unsigned mx = (unsigned)(d.get_scal(SC_AUX) & 0xffffffffu); // the arc of a hit within its read is never longer than the read (miniasm.h:97-98); the kernels flag the others
+	uint32_t lb = bits_for(mx);
 	if (h.n) {
 		if (h.n >= (1ull << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 arcs on one GPU\n"); exit(73); }
 		static const bool seg_sort = !(getenv("MAB_SG_SEGSORT") && atoi(getenv("MAB_SG_SEGSORT")) == 0); // default on; 0 = device-wide column sort
 		uint32_t n_del = 0;
-		if (seg_sort && sg_emit_segmented(d, h, p, lb, g, &n_del)) return n_del;
+		if (seg_sort && sg_emit_segmented(d, h, len, p, lb, g, &n_del)) return n_del;
 		dh_hits_dense(d, h);
-		d.zero_scal(SC_COUNT);
-		const uint64_t sentinel = 1ull << (lb + bits_for((uint64_t)n_seq * 2 - 1));
 		uint64_t *ka = mab_alloc<uint64_t>(d, h.n), *kb = mab_alloc<uint64_t>(d, h.n), *va = mab_alloc<uint64_t>(d, h.n), *vb = mab_alloc<uint64_t>(d, h.n);
-		// seq lengths are read while other threads may set del bits: lengths are masked, so this is benign
-		MAB_LAUNCH(d, k_sg_arcs, mab_grid(h.n, 256), 256, 0, h.a, h.n, g.seq, p, lb, sentinel, ka, va, d.d_scal + SC_COUNT);
-		const uint32_t n_arc = (uint32_t)d.get_scal(SC_COUNT);
+		uint32_t n_arc;
+		for (;;) { // lb bounds the arcs of hits that lie within their reads; one past its read's end takes the full 32 bits
+			d.zero_scal(SC_COUNT);
+			d.zero_scal(SC_AUX);
+			const uint64_t sentinel = 1ull << (lb + bits_for((uint64_t)n_seq * 2 - 1));
+			MAB_LAUNCH(d, k_sg_arcs, mab_grid(h.n, 256), 256, 0, h.a, h.n, len, g.seq, p, lb, sentinel, ka, va, d.d_scal + SC_COUNT, d.d_scal + SC_AUX);
+			n_arc = (uint32_t)d.get_scal(SC_COUNT);
+			if (!d.h_scal[SC_AUX]) break;
+			lb = 32;
+		}
 		dg_build_sorted(d, g, ka, va, kb, vb, (uint32_t)h.n, n_arc, lb, true);
 		d.free(ka); d.free(kb); d.free(va); d.free(vb);
 	} else { dg_reserve(d, g, 1); g.is_srt = true; }

@@ -449,7 +449,9 @@ asg_t *ma_sg_gen(const ma_opt_t *opt, const sdict_t *d, const ma_sub_t *sub, siz
 		const ma_hit_t *h = &hit[i];
 		uint32_t q = (uint32_t)(h->qns >> 32);
 		asg_arc_t t;
-		int r = hit2arc(h, (int)g->seq[q].len, (int)g->seq[h->tn].len, opt->max_hang, opt->int_frac, opt->min_ovlp, &t);
+		/* the 32-bit lengths (asm.c:23-24): asg_seq_t::len keeps only 31 bits of them */
+		int ql = sub ? (int)(sub[q].e - sub[q].s) : (int)d->seq[q].len, tl = sub ? (int)(sub[h->tn].e - sub[h->tn].s) : (int)d->seq[h->tn].len;
+		int r = hit2arc(h, ql, tl, opt->max_hang, opt->int_frac, opt->min_ovlp, &t);
 		if (r >= 0) {
 			if (q == h->tn) { if ((uint32_t)h->qns == h->ts && h->qe == h->te && h->rev) g->seq[q].del = 1; }
 			else *arc_push(g) = t;

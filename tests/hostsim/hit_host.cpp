@@ -36,15 +36,15 @@ size_t hs_hit_flt(const DSub *sub, int max_hang, int min_ovlp, size_t n, DHit *a
 }
 
 // the arc-emission loop of ma_sg_gen (asm.c:14-36) before asg_cleanup: arcs in hit order, seq[i] = len | del<<31.
-// `seq` comes in holding the lengths and deletion flags of asm.c:14-17.
-size_t hs_sg_arcs(int max_hang, float int_frac, int min_ovlp, size_t n, const DHit *a, uint32_t *seq, DArc *out)
+// `seq` comes in holding the lengths and deletion flags of asm.c:14-17; len32 the 32-bit lengths the classifier takes (asm.c:23-24).
+size_t hs_sg_arcs(int max_hang, float int_frac, int min_ovlp, size_t n, const DHit *a, const uint32_t *len32, uint32_t *seq, DArc *out)
 {
 	size_t m = 0;
 	for (size_t i = 0; i < n; ++i) {
 		const DHit h = a[i];
 		const uint32_t qn = (uint32_t)(h.qns >> 32);
 		DArc t;
-		const int r = mab_hit2arc(h, (int)(seq[qn] & 0x7fffffffu), (int)(seq[h.tn] & 0x7fffffffu), max_hang, int_frac, min_ovlp, &t);
+		const int r = mab_hit2arc(h, (int)len32[qn], (int)len32[h.tn], max_hang, int_frac, min_ovlp, &t);
 		if (r >= 0) {
 			if (qn == h.tn) {
 				if ((uint32_t)h.qns == h.ts && h.qe == h.te && (h.ml_rev >> 31)) seq[qn] |= MAB_DEL_BIT;

@@ -34,7 +34,7 @@ def sim(built):
     dll.hs_hit_cut.restype, dll.hs_hit_cut.argtypes = C.c_size_t, [C.c_void_p, C.c_int, C.c_size_t, C.c_void_p]
     dll.hs_hit_flt.restype, dll.hs_hit_flt.argtypes = C.c_size_t, [C.c_void_p, C.c_int, C.c_int, C.c_size_t, C.c_void_p, C.POINTER(C.c_ulonglong)]
     dll.hs_sg_arcs.restype = C.c_size_t
-    dll.hs_sg_arcs.argtypes = [C.c_int, C.c_float, C.c_int, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
+    dll.hs_sg_arcs.argtypes = [C.c_int, C.c_float, C.c_int, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     dll.hs_comp.restype, dll.hs_comp.argtypes = C.c_ubyte, [C.c_ubyte]
     dll.hs_hit2arc.restype = C.c_int
     dll.hs_hit2arc.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_void_p]
@@ -73,13 +73,19 @@ def layout_hits(rng, sub, n):
 def fuzz(seed, n_seq=64, n=20000, wild=True):
     """Random interval table and hits.  wild=False keeps every hit inside the kept intervals (what the later stages see after
     ma_hit_cut); wild=True lets coordinates fall anywhere, spans wrap and intervals be empty or deleted; wild="layout": hits of a
-    consistent layout (layout_hits), coordinates relative to the kept intervals."""
+    consistent layout (layout_hits), coordinates relative to the kept intervals; wild="long": as True, and a quarter of the
+    intervals start near 2^31 and end small, so that their 32-bit length e - s is 2^31 or more (a second-round interval whose
+    start went below zero, hit.c:148)."""
     rng = np.random.default_rng(seed)
     s = rng.integers(0, 4000, n_seq).astype(np.uint32)
     ln = rng.integers(0, 14000, n_seq).astype(np.uint32)
     ln[rng.random(n_seq) < 0.05] = 0                                    # empty kept interval
     sub = np.zeros(n_seq, dtype=SUB_DT)
     sub["s_del"], sub["e"] = s, s + ln
+    if wild == "long":
+        far = rng.random(n_seq) < 0.25
+        sub["s_del"][far] = (np.uint32(1 << 31) - rng.integers(1, 1000, int(far.sum()))).astype(np.uint32)
+        sub["e"][far] = rng.integers(0, 14000, int(far.sum())).astype(np.uint32)
     if wild == "layout":
         return sub, layout_hits(rng, sub, n)
     if wild:
@@ -88,10 +94,10 @@ def fuzz(seed, n_seq=64, n=20000, wild=True):
     q, t = rng.integers(0, n_seq, n), rng.integers(0, n_seq, n)
     same = rng.random(n) < 0.03
     t[same] = q[same]                                                   # self hits
-    base_q = np.where(wild, 0, 0) + (sub["s_del"][q] & 0x7fffffff if wild else 0)
+    base_q = (sub["s_del"][q] & 0x7fffffff).astype(np.int64) if wild else np.zeros(n, dtype=np.int64)
     lim_q = (sub["e"][q] if wild else ln[q]).astype(np.int64)
     lim_t = (sub["e"][t] if wild else ln[t]).astype(np.int64)
-    base_t = (sub["s_del"][t] & 0x7fffffff) if wild else np.zeros(n, dtype=np.int64)
+    base_t = (sub["s_del"][t] & 0x7fffffff).astype(np.int64) if wild else np.zeros(n, dtype=np.int64)
 
     def span(base, lim):
         a = base + rng.integers(-2500 if wild else 0, 6000, n)
@@ -133,8 +139,18 @@ def test_cut(seed, min_span, ref, sim):
 
 
 @pytest.mark.parametrize("seed", range(6))
+@pytest.mark.parametrize("min_span", [1, 2000])
+def test_cut_long(seed, min_span, ref, sim):
+    sub, h = fuzz(400 + seed, wild="long")
+    a, b = h.copy(), h.copy()
+    na = ref.ma_hit_cut(_ptr(sub), min_span, len(a), _ptr(a))
+    nb = sim.hs_hit_cut(_ptr(sub), min_span, len(b), _ptr(b))
+    assert na == nb and np.array_equal(a[:na], b[:nb])
+
+
+@pytest.mark.parametrize("seed", range(6))
 @pytest.mark.parametrize("max_hang,min_ovlp", [(1500, 1000), (0, 0), (50, 5000), (100000, 1), (700, 20000)])
-@pytest.mark.parametrize("wild", [False, True, "layout"])
+@pytest.mark.parametrize("wild", [False, True, "layout", "long"])
 def test_flt(seed, max_hang, min_ovlp, wild, ref, sim):
     sub, h = fuzz(100 + seed, wild=wild)
     a, b = h.copy(), h.copy()
@@ -155,7 +171,7 @@ def test_flt(seed, max_hang, min_ovlp, wild, ref, sim):
 
 @pytest.mark.parametrize("seed", range(6))
 @pytest.mark.parametrize("max_hang,int_frac,min_ovlp", [(1000, 0.8, 2000), (0, 0.8, 2000), (1000, 0.0, 0), (1000, 1.0, 2000), (30000, 0.3, 1), (200, 0.95, 12000)])
-@pytest.mark.parametrize("wild", [False, True, "layout"])
+@pytest.mark.parametrize("wild", [False, True, "layout", "long"])
 def test_sg_gen(seed, max_hang, int_frac, min_ovlp, wild, ref, sim):
     sub, h = fuzz(200 + seed, wild=wild)
     n_seq = len(sub)
@@ -168,10 +184,10 @@ def test_sg_gen(seed, max_hang, int_frac, min_ovlp, wild, ref, sim):
     arcs_r, seq_r, _, _, _ = ref.read_graph(g)
     ref.asg_destroy(g), ref.sd_destroy(d)
 
-    seq = ((sub["e"] - (sub["s_del"] & np.uint32(0x7fffffff))) & np.uint32(0x7fffffff)) | (sub["s_del"] & DEL)   # asm.c:14-17
-    seq = seq.astype(np.uint32)
+    len32 = (sub["e"] - (sub["s_del"] & np.uint32(0x7fffffff))).astype(np.uint32)                              # asm.c:23-24
+    seq = ((len32 & np.uint32(0x7fffffff)) | (sub["s_del"] & DEL)).astype(np.uint32)                            # asm.c:14-17
     out = np.zeros(len(h), dtype=ARC_DT)
-    m = sim.hs_sg_arcs(max_hang, int_frac, min_ovlp, len(h), _ptr(h), _ptr(seq), _ptr(out))
+    m = sim.hs_sg_arcs(max_hang, int_frac, min_ovlp, len(h), _ptr(h), _ptr(len32), _ptr(seq), _ptr(out))
     arcs = out[:m]
     assert np.array_equal(seq, seq_r)
     dead = (seq & DEL) != 0                                              # asg_cleanup: asg_arc_rm + sort (asg.c:57-80)
@@ -194,6 +210,24 @@ def test_fuzz_reaches_every_class(sim):
             seen[key] = seen.get(key, 0) + 1
     for cls in (-1, -2, -3, -4, ("arc", 0, 0), ("arc", 0, 1), ("arc", 1, 0), ("arc", 1, 1)):
         assert seen.get(cls, 0) > 0, (cls, seen)
+
+
+def test_long_fuzz_needs_the_32_bit_lengths(sim):
+    """With wild="long" the 32-bit length of many intervals is 2^31 or more; for a share of the hits on them ma_hit2arc gives
+    another class or another arc with that length than with the 31-bit asg_seq_t::len, so test_sg_gen tells the two apart."""
+    sub, h = fuzz(500, wild="long")
+    len32 = (sub["e"] - (sub["s_del"] & np.uint32(0x7fffffff))).astype(np.uint32)
+    assert (len32 >= np.uint32(1 << 31)).sum() >= 8
+    t32, t31 = np.zeros(1, dtype=ARC_DT), np.zeros(1, dtype=ARC_DT)
+    differ = 0
+    for i in range(0, len(h), 3):
+        q, t = int(h["qns"][i]) >> 32, int(h["tn"][i])
+        if len32[q] < 1 << 31 and len32[t] < 1 << 31:
+            continue
+        r32 = sim.hs_hit2arc(_ptr(h[i:i + 1]), int(len32[q].astype(np.int32)), int(len32[t].astype(np.int32)), 1000, 0.8, 2000, _ptr(t32))
+        r31 = sim.hs_hit2arc(_ptr(h[i:i + 1]), int(len32[q]) & 0x7fffffff, int(len32[t]) & 0x7fffffff, 1000, 0.8, 2000, _ptr(t31))
+        differ += r32 != r31 or (r32 >= 0 and t32.tobytes() != t31.tobytes())
+    assert differ >= 20, differ
 
 
 def test_complement_of_every_byte(ref, sim, tmp_path):
