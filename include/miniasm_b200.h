@@ -173,6 +173,24 @@ size_t mab_paf_text(const mab_ctx_t *ctx, char *dst, size_t cap);
 int mab_ingest(mab_ctx_t *ctx, int min_span, int min_match, int bi_dir);
 /* load + ingest overlapped: chunks of the host text are parsed while the next ones cross PCIe (same result as the two calls) */
 int mab_load_ingest_text(mab_ctx_t *ctx, const char *text, size_t len, int min_span, int min_match, int bi_dir);
+/* Step 1 without the text in HBM: the PAF is taken from a source in windows of window_bytes (0 = 256 MB; at least 64 KB; a
+ * longer line grows the windows) and read twice -- names, ids and hit counts first, then the hits straight into their sorted
+ * place -- so the device holds two windows, the read names and the hits, whatever the size of the text.  Leaves the state
+ * mab_ingest leaves (a text loaded before is dropped).  The source must deliver the same bytes after rewind: a difference
+ * ends the process with exit code 78.  Returns 0; mab_ingest_windowed -1 when rewind fails (nothing ingested, the context stays
+ * usable); mab_ingest_file_windowed -1 when the file cannot be opened and -2 when it cannot be rewound ("-" on a pipe).  A
+ * gzip file is inflated by zlib on the host here, twice. */
+typedef struct {
+	size_t (*read)(void *ud, char *dst, size_t cap);  /* next bytes in order, 0 at the end */
+	int    (*rewind)(void *ud);                       /* back to byte 0; -1 if impossible */
+	void   *ud;
+} mab_text_source_t;
+int mab_ingest_windowed(mab_ctx_t *ctx, const mab_text_source_t *src, size_t window_bytes, int min_span, int min_match, int bi_dir);
+int mab_ingest_file_windowed(mab_ctx_t *ctx, const char *fn, size_t window_bytes, int min_span, int min_match, int bi_dir);
+/* high-water mark, in bytes, of the device memory the context's allocator handed out; reset != 0 restarts it at the current use */
+size_t mab_mem_peak(mab_ctx_t *ctx, int reset);
+/* device memory, in bytes, the context could still take: what the driver reports free plus what its allocator holds unused */
+size_t mab_mem_free(mab_ctx_t *ctx);
 /* -R: ma_hit_no_cont (hit.c:38-68) + ma_hit_read with its exclusion list (hit.c:86) as one pass over the resident text */
 int mab_ingest_nocont(mab_ctx_t *ctx, int min_span, int min_match, int bi_dir, int max_hang, float int_frac);
 /* alternative to load+ingest: hits and dictionary produced by the drop-in ma_hit_read (host arrays) */

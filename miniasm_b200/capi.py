@@ -131,6 +131,14 @@ class MabStats(C.Structure):                                          # mab_stat
                [(n, C.c_double) for n in ("ms_ingest", "ms_select", "ms_layout", "ms_unitigs")]
 
 
+MAB_READ_FN = C.CFUNCTYPE(C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t)   # mab_text_source_t::read
+MAB_REWIND_FN = C.CFUNCTYPE(C.c_int, C.c_void_p)                            # mab_text_source_t::rewind
+
+
+class MabTextSource(C.Structure):                                     # mab_text_source_t
+    _fields_ = [("read", MAB_READ_FN), ("rewind", MAB_REWIND_FN), ("ud", C.c_void_p)]
+
+
 # symbols include/miniasm_b200.h declares beyond the reference seam
 _PRODUCT_ONLY = {
     "mab_create": (C.c_void_p, [C.c_int]),
@@ -142,6 +150,10 @@ _PRODUCT_ONLY = {
     "mab_paf_text": (C.c_size_t, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "mab_ingest": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int]),
     "mab_load_ingest_text": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int]),
+    "mab_ingest_windowed": (C.c_int, [C.c_void_p, C.POINTER(MabTextSource), C.c_size_t, C.c_int, C.c_int, C.c_int]),
+    "mab_ingest_file_windowed": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t, C.c_int, C.c_int, C.c_int]),
+    "mab_mem_peak": (C.c_size_t, [C.c_void_p, C.c_int]),
+    "mab_mem_free": (C.c_size_t, [C.c_void_p]),
     "mab_ingest_nocont": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
     "mab_load_hits": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(Sdict)]),
     "mab_select": (C.c_int, [C.c_void_p, C.POINTER(MaOpt), C.c_int, C.c_int, C.c_int]),

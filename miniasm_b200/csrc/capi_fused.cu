@@ -16,6 +16,7 @@
 #include <map>
 #include <string>
 #include <zlib.h>
+#include <errno.h>
 #include <fcntl.h>
 #include <unistd.h>
 #include <sys/stat.h>
@@ -411,6 +412,81 @@ int mab_load_ingest_text(mab_ctx_t *c, const char *text, size_t len, int min_spa
 		fprintf(stderr, "[M::%s::%s] read %ld hits; stored %ld hits and %d sequences (%ld bp)\n", "ma_hit_read", sys_timestamp(),
 				(long)c->ist.n_parsed, (long)c->ist.n_hits, (int)c->ist.n_seq, (long)c->ist.tot_len);
 	return 0;
+}
+
+/* ---- Step 1 in windows: the text never becomes resident (ingest_paf_windowed, DESIGN.md 3d) ---------------------------- */
+static int ingest_windowed(mab_ctx *c, const TextSource &src, size_t window_bytes, size_t size_hint, int min_span, int min_match, int bi_dir)
+{
+	MAB_CUDA(cudaSetDevice(c->dev.device));
+	MabDev &d = c->dev;
+	PhaseTimer pt(d, &c->stats.ms_ingest, "mab_ingest_windowed");
+	ctx_reset_reads(c);
+	d.free(c->d_text), c->d_text = nullptr, c->text_len = c->text_cap = 0; // a text loaded earlier is given up: this ingest keeps names, not text
+	if (!ingest_paf_windowed(d, src, window_bytes ? window_bytes : (size_t)256 << 20, size_hint, min_span, min_match, bi_dir, c->hits, c->names, &c->name_text, c->ist))
+		return -1;
+	c->n_seq = c->names.n_seq;
+	c->stats.n_lines = c->ist.n_parsed, c->stats.n_hits_stored = c->ist.n_hits, c->stats.n_seq_in = c->ist.n_seq;
+	if (!mab_mute && ma_verbose >= 3)
+		fprintf(stderr, "[M::%s::%s] read %ld hits; stored %ld hits and %d sequences (%ld bp)\n", "ma_hit_read", sys_timestamp(),
+				(long)c->ist.n_parsed, (long)c->ist.n_hits, (int)c->ist.n_seq, (long)c->ist.tot_len);
+	return 0;
+}
+
+int mab_ingest_windowed(mab_ctx_t *c, const mab_text_source_t *src, size_t window_bytes, int min_span, int min_match, int bi_dir)
+{
+	const TextSource ts = { src->read, src->rewind, src->ud };
+	return ingest_windowed(c, ts, window_bytes, 0, min_span, min_match, bi_dir);
+}
+
+struct FileSource { int fd; gzFile gz; }; // a plain file is read and sought directly, a gzip file through zlib on the host
+
+static size_t file_read(void *ud, char *dst, size_t cap)
+{
+	FileSource *f = (FileSource*)ud;
+	if (f->gz) { const int r = gzread(f->gz, dst, (unsigned)(cap < (1u << 30) ? cap : (1u << 30))); return r > 0 ? (size_t)r : 0; }
+	ssize_t r;
+	do r = read(f->fd, dst, cap); while (r < 0 && errno == EINTR);
+	return r > 0 ? (size_t)r : 0;
+}
+
+static int file_rewind(void *ud)
+{
+	FileSource *f = (FileSource*)ud;
+	return f->gz ? gzrewind(f->gz) : lseek(f->fd, 0, SEEK_SET) == 0 ? 0 : -1;
+}
+
+int mab_ingest_file_windowed(mab_ctx_t *c, const char *fn, size_t window_bytes, int min_span, int min_match, int bi_dir)
+{
+	FileSource f = { fn && strcmp(fn, "-") ? open(fn, O_RDONLY) : dup(fileno(stdin)), nullptr };
+	if (f.fd < 0) return -1;
+	struct stat sb;
+	uint8_t mg[2];
+	size_t hint = fstat(f.fd, &sb) == 0 && S_ISREG(sb.st_mode) ? (size_t)sb.st_size : 0;
+	if (hint && pread(f.fd, mg, 2, 0) == 2 && gz_magic(mg, 2)) {
+		f.gz = gzdopen(f.fd, "r");
+		if (f.gz == 0) { close(f.fd); return -1; }
+		gzbuffer(f.gz, 1 << 20);
+		hint *= 4;                                   // (a guess at the inflated size: it only sizes the first dictionary)
+	}
+	const TextSource ts = { file_read, file_rewind, &f };
+	const int rc = ingest_windowed(c, ts, window_bytes, hint, min_span, min_match, bi_dir);
+	if (f.gz) gzclose(f.gz); else close(f.fd);
+	return rc < 0 ? -2 : 0;
+}
+
+size_t mab_mem_peak(mab_ctx_t *c, int reset)
+{
+	const size_t p = c->dev.arena.peak;
+	if (reset) c->dev.arena.peak = c->dev.arena.in_use;
+	return p;
+}
+
+size_t mab_mem_free(mab_ctx_t *c)
+{
+	size_t fr = 0, tot = 0;
+	MAB_CUDA(cudaSetDevice(c->dev.device));
+	MAB_CUDA(cudaMemGetInfo(&fr, &tot));
+	return fr + (c->dev.arena.reserved - c->dev.arena.in_use);
 }
 
 /* -R (main.c:110-113 + hit.c:38-68,86): Step 0 and Step 1 in one pass over the text that is already in HBM.  Prints the

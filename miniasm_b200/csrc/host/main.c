@@ -138,10 +138,29 @@ static mab_ctx_t *run_sharded(const char *fn, const ma_opt_t *opt, int bi_dir, i
 	return ctx0;
 }
 
+/* MINIASM_B200_INGEST=auto: does Step 1 take the windowed ingest?  Only for a plain regular file whose text and line arrays
+ * (what the resident ingest holds beside the hits: the padded text, a line start and a 32-byte record per estimated line) would
+ * take more than half of the free device memory -- inputs the resident ingest cannot hold.  The half is a guess, not a measurement. */
+static int auto_windowed(mab_ctx_t *ctx, const char *fn)
+{
+	struct stat sb;
+	unsigned char magic[2] = {0, 0};
+	int fd, plain;
+	size_t len;
+	if (strcmp(fn, "-") == 0 || (fd = open(fn, O_RDONLY)) < 0) return 0;
+	plain = fstat(fd, &sb) == 0 && S_ISREG(sb.st_mode) && !(pread(fd, magic, 2, 0) == 2 && magic[0] == 0x1f && magic[1] == 0x8b);
+	close(fd);
+	if (!plain) return 0;
+	len = (size_t)sb.st_size;
+	return len / 8 * 9 + 40 * (len / 24 + 1024) > mab_mem_free(ctx) / 2;
+}
+
 int main(int argc, char *argv[])
 {
 	ma_opt_t opt;
 	int i, c, stage = 100, no_first = 0, no_second = 0, bi_dir = 1, o_set = 0, no_cont = 0, device = 0, n_gpus = 1, sharded_done = 0, gpu_seq = 0;
+	int windowed = -1;           /* MINIASM_B200_INGEST: 1 windowed, 0 resident, -1 auto */
+	size_t window_bytes = 0;     /* MINIASM_B200_WINDOW (0: the library's default) */
 	const char *fn_reads = 0, *outfmt = "ug", *env;
 	mab_ctx_t *ctx;
 	FILE *out = stdout;          /* where the GFA goes */
@@ -190,6 +209,14 @@ int main(int argc, char *argv[])
 		fprintf(stderr, "[W::%s] MINIASM_B200_GPUS=%d covers the default pipeline (-p ug|sg without -R/-1/-2/-S/-f): running on one GPU\n", __func__, n_gpus);
 		n_gpus = 1;
 	}
+	if ((env = getenv("MINIASM_B200_INGEST")) != 0) windowed = strcmp(env, "windowed") == 0 ? 1 : strcmp(env, "resident") == 0 ? 0 : -1;
+	if ((env = getenv("MINIASM_B200_WINDOW")) != 0) window_bytes = (size_t)strtoull(env, 0, 10);
+	if (windowed == 1 && (no_cont || n_gpus > 1 || strcmp(argv[optind], "-") == 0)) { /* (auto never picks it for these) */
+		fprintf(stderr, "[W::%s] MINIASM_B200_INGEST=windowed does not cover %s: the PAF text is loaded whole\n", __func__,
+		        no_cont ? "-R" : n_gpus > 1 ? "MINIASM_B200_GPUS" : "standard input, which cannot be read twice");
+		windowed = 0;
+	}
+	if (no_cont || n_gpus > 1) windowed = 0;
 	if (n_gpus > 1) { /* steps 1-4 sharded; what follows (unitigs, output) runs on rank 0's context as in a single-GPU run */
 		/* stdout carries the GFA and NCCL prints its version banner (NCCL_DEBUG=VERSION) there: the GFA keeps the original
 		 * descriptor, everything else that writes to fd 1 from here on lands on stderr */
@@ -217,12 +244,16 @@ int main(int argc, char *argv[])
 		}
 		mab_ingest_nocont(ctx, opt.min_span, opt.min_match, bi_dir, opt.max_hang, opt.int_frac);
 	} else {
+		int rc = -2;                 /* -2: the windowed ingest did not run */
 		fprintf(stderr, "[M::%s] ===> Step 1: reading read mappings <===\n", __func__);
-		if (mab_load_paf_file(ctx, argv[optind]) < 0) {
+		if (windowed < 0) windowed = auto_windowed(ctx, argv[optind]);
+		if (windowed) rc = mab_ingest_file_windowed(ctx, argv[optind], window_bytes, opt.min_span, opt.min_match, bi_dir);
+		if (rc == -2 && windowed) fprintf(stderr, "[W::%s] %s cannot be read twice: the PAF text is loaded whole\n", __func__, argv[optind]);
+		if (rc == -1 || (rc == -2 && mab_load_paf_file(ctx, argv[optind]) < 0)) {
 			fprintf(stderr, "[E::%s] could not open PAF file %s\n", "ma_hit_read", argv[optind]);
 			exit(1);
 		}
-		mab_ingest(ctx, opt.min_span, opt.min_match, bi_dir);
+		if (rc == -2) mab_ingest(ctx, opt.min_span, opt.min_match, bi_dir);
 	}
 
 	if (!sharded_done) mab_select(ctx, &opt, no_first, no_second, stage); /* prints the Step 2 / Step 3 banners where the reference does */

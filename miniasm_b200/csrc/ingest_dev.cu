@@ -1354,3 +1354,482 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 	dh_sort(d, h);
 	d.trace("shard-ingest:sort");
 }
+
+// =============================================================================================================
+// Windowed ingest: the text comes from a source that is read twice, one window at a time, so the device never holds more
+// of it than two windows (DESIGN.md 3d).  A window is a run of whole lines: it is numbered, parsed and filtered the way
+// k_parse_tiles does it (8 KB tiles staged in shared memory, decoupled look-back over the window's tiles), with the global
+// number of the window's first line carried from window to window in device memory.
+//   pass 1  enters the names of the stored lines into the dictionary and counts the hits per name; no record is kept.  A
+//           name that is new is copied into the packed name store at once and its witness re-pointed there, so nothing
+//           refers to a window after its launch; first[slot] carries the sequence-length column of the occurrence it names.
+//   pass 2  parses the same windows again, looks the names up and writes every hit and its mirror straight into its read's
+//           bucket with the ordinal 2 * line (+ 1), as k_hit_emit does.
+// =============================================================================================================
+// device words of a windowed run; the two pairs (line, bl) are adjacent so that one copy hands OUT to the next window's IN
+enum { WS_PARSED = 0, WS_STORED, WS_TAB_FULL, WS_STORE_FULL, WS_STORE_USED, WS_BAD, WS_EMITTED,
+       WS_LINE_IN, WS_BL_IN,    // global number of the window's first line; (1 + line) << 31 | bl of the last line with an 11th field before the window
+       WS_LINE_OUT, WS_BL_OUT,  // the same after the window
+       WS_N };
+
+struct WinTab {
+	NameTab t;                   // key: witness offsets count through the name store first, then through the current window;
+	                             // first: (2 * line + role) << 32 | sequence-length column of that occurrence
+	char *store;                 // names of the dictionary, each followed by a TAB
+	uint64_t store_cap;
+};
+
+// (pass 1 reads witnesses past the L1: a name stored by another CTA of the same launch may share a line with bytes cached before)
+template <bool CG>
+__device__ __forceinline__ bool name_at(const char *w, const char *nm, uint32_t nl)
+{
+	for (uint32_t i = 0; i < nl; ++i) if ((CG ? __ldcg(w + i) : w[i]) != nm[i]) return false;
+	return (CG ? __ldcg(w + nl) : w[nl]) == '\t';
+}
+
+// name = nm[0 .. nl), followed by a TAB, at byte woff of the window `win`; occ = 2 * line + role, slen = its length column
+__device__ __forceinline__ uint32_t win_insert(const WinTab &t, const char *win, const char *nm, uint32_t nl, uint64_t woff, uint64_t occ, uint32_t slen,
+                                               unsigned long long *ws)
+{
+	const uint64_t h = name_hash(nm, 0, nl, 0);
+	const unsigned long long frag = (h >> 37) << NT_OFF_BITS, mine = frag | (t.store_cap + woff + 1);
+	uint64_t s = h & t.t.mask;
+	for (int probe = 0; probe < 1 << 14; ++probe, s = (s + 1) & t.t.mask) {
+		unsigned long long k = t.t.key[s];
+		bool fresh = false;
+		if (k == 0) {
+			k = atomicCAS(&t.t.key[s], 0ull, mine);
+			if (k == 0) k = mine, fresh = true;
+		}
+		if ((k ^ mine) >> NT_OFF_BITS) continue;                      // another fragment
+		if (fresh) { // a new name: into the store, then the witness points there (until then it points at this occurrence, which stays put for the launch)
+			const unsigned long long at = atomicAdd(ws + WS_STORE_USED, (unsigned long long)nl + 1);
+			if (at + nl + 1 <= t.store_cap) {
+				for (uint32_t i = 0; i < nl; ++i) t.store[at + i] = nm[i];
+				t.store[at + nl] = '\t';
+				__threadfence();
+				atomicExch(&t.t.key[s], frag | (at + 1));
+			} else atomicAdd(ws + WS_STORE_FULL, 1ull);
+		} else {
+			const uint64_t off = (k & NT_OFF_MASK) - 1;
+			if (!name_at<true>(off < t.store_cap ? t.store + off : win + (off - t.store_cap), nm, nl)) continue;
+		}
+		const unsigned long long v = occ << 32 | slen;
+		if (t.t.first[s] > v) atomicMin(&t.t.first[s], v);
+		return (uint32_t)s;
+	}
+	atomicAdd(ws + WS_TAB_FULL, 1ull);
+	return 0;
+}
+
+// pass 2: the slot of a name, NOSLOT when the dictionary of pass 1 does not have it
+__device__ __forceinline__ uint32_t win_find(const WinTab &t, const char *nm, uint32_t nl)
+{
+	const uint64_t h = name_hash(nm, 0, nl, 0);
+	uint64_t s = h & t.t.mask;
+	for (int probe = 0; probe < 1 << 14; ++probe, s = (s + 1) & t.t.mask) {
+		const unsigned long long k = t.t.key[s];
+		if (k == 0) break;
+		if ((k >> NT_OFF_BITS) == (h >> 37) && name_at<false>(t.store + ((k & NT_OFF_MASK) - 1), nm, nl)) return (uint32_t)s;
+	}
+	return NOSLOT;
+}
+
+// bl of the 10-field line that starts at byte s of the window: the 11th column of the closest earlier line that has one
+// (paf.c:47, hit.c:73), searched backwards through the window, then what the windows before left behind
+__device__ uint32_t win_prev_bl(const char *text, uint64_t s, unsigned long long carry)
+{
+	while (s > 0) {
+		uint64_t eol = s - 1, p = eol;                                // text[eol] is the '\n' that ends the line before
+		while (p > 0 && text[p - 1] != '\n') --p;
+		if (eol - p > 1 && text[eol - 1] == '\r') --eol;
+		uint64_t q = p;
+		int tabs = 0;
+		for (; q < eol && tabs < 10; ++q) tabs += text[q] == '\t';
+		if (tabs == 10) {
+			uint64_t f = q;
+			while (f < eol && text[f] != '\t') ++f;
+			return num_field(text + q, 0, (uint32_t)(f - q)) & 0x7fffffffu;
+		}
+		s = p;
+	}
+	return (uint32_t)carry & 0x7fffffffu;
+}
+
+// One window [text, text + len) of whole lines (the last window may lack the final '\n'), one tile per CTA.
+// PASS 2: bfirst = bucket starts per read id (n_seq + 1), cur = fill cursors, out = the hit buckets.
+template <int PASS>
+__global__ void __launch_bounds__(PT_THREADS)
+k_win_tiles(const char *__restrict__ text, size_t len, unsigned *tile_ctr, LineTileState tstate, int min_span, int min_match, int bi_dir, WinTab tab,
+            const uint32_t *__restrict__ bfirst, uint32_t *cur, DHit *out, unsigned long long *ws)
+{
+	typedef cub::BlockScan<uint32_t, PT_THREADS> BS;
+	__shared__ __align__(16) char s_text[PT_TILE + PT_OVER + 16];
+	__shared__ uint16_t s_start[PT_LIST + 1];
+	__shared__ uint32_t s_vals[PT_THREADS / 32][11][32];
+	__shared__ typename BS::TempStorage s_scan;
+	__shared__ typename LinePrefixOp::TempStorage s_pref;
+	__shared__ unsigned long long s_first, s_tile, s_eol;
+	__shared__ uint32_t s_nl;
+	const uint32_t lane = threadIdx.x & 31;
+	if (threadIdx.x == 0) s_tile = atomicAdd(tile_ctr, 1u), s_nl = ~0u;
+	__syncthreads();
+	const uint64_t t = s_tile, b0 = t * PT_TILE, b1 = b0 + PT_TILE < len ? b0 + PT_TILE : len;
+	const uint64_t w_end = b1 + PT_OVER < len ? b1 + PT_OVER : len;           // staged bytes: [b0, w_end)
+	{
+		const uint32_t n16 = (uint32_t)((w_end - b0 + 15) >> 4);  // the tail word may reach past `len` but stays inside the (padded) window
+		for (uint32_t k = threadIdx.x; k < n16; k += PT_THREADS)
+			reinterpret_cast<uint4*>(s_text)[k] = __ldg(reinterpret_cast<const uint4*>(text + b0) + k);
+	}
+	__syncthreads();
+	const uint32_t my0 = threadIdx.x * 64, lim = (uint32_t)((b1 == len ? len - 1 : b1) - b0);
+	uint64_t bits = 0;
+	#pragma unroll
+	for (int k = 0; k < 4; ++k) bits |= (uint64_t)nl_bits_u4(reinterpret_cast<const uint4*>(s_text + my0)[k]) << (16 * k);
+	bits &= lim <= my0 ? 0ull : lim - my0 >= 64 ? ~0ull : (1ull << (lim - my0)) - 1;
+	const bool line0 = t == 0 && threadIdx.x == 0;            // the window's first line starts at its byte 0
+	uint32_t rank, n;
+	BS(s_scan).ExclusiveSum((uint32_t)__popcll(bits) + line0, rank, n);
+	for (uint32_t o = lim + threadIdx.x; o < (uint32_t)(w_end - b0); o += PT_THREADS)
+		if (s_text[o] == '\n' && b0 + o < len) { atomicMin(&s_nl, o); break; }
+	if (threadIdx.x < 32) {
+		if (t == 0) {
+			if (threadIdx.x == 0) tstate.SetInclusive(0, n), s_first = 0;
+		} else {
+			LinePrefixOp op(tstate, s_pref, ::cuda::std::plus<unsigned long long>(), (int)t);
+			const unsigned long long ex = op(n);
+			if (threadIdx.x == 0) s_first = ex;
+		}
+	}
+	__syncthreads();
+	const uint64_t first = ws[WS_LINE_IN] + s_first;          // global number of the tile's first line
+	if (threadIdx.x == 0 && b1 == len) ws[WS_LINE_OUT] = first + n;
+	if (n == 0) return;
+	uint64_t last_eol = s_nl != ~0u ? b0 + s_nl : w_end >= len ? len : ~0ull; // ~0: the tile's last line ends past the overhang
+	if (last_eol == ~0ull) {
+		if (threadIdx.x < 32) {
+			uint64_t e = len;
+			for (uint64_t p = w_end; p < len; p += 32 * 16) {
+				const uint64_t q = p + 16 * lane;
+				uint32_t m = 0;
+				for (uint32_t k = 0; k < 16 && q + k < len; ++k) m |= (uint32_t)(text[q + k] == '\n') << k;
+				const unsigned hit = __ballot_sync(0xffffffffu, m != 0);
+				if (hit) { e = __shfl_sync(0xffffffffu, q + __ffs(m) - 1, __ffs(hit) - 1); break; }
+			}
+			if (threadIdx.x == 0) s_eol = e;
+		}
+		__syncthreads();
+		last_eol = s_eol;
+	}
+	unsigned n_parsed = 0, n_pass = 0, n_bad = 0, n_emit = 0;
+	unsigned long long last11 = 0;                            // (1 + line) << 31 | bl of this thread's last line with an 11th field
+	for (uint32_t r0 = 0; r0 < n; r0 += PT_LIST) {
+		{
+			uint32_t r = rank;
+			uint64_t b = bits;
+			if (line0) { if (r == r0) s_start[0] = 0; ++r; }
+			for (; b && r <= r0 + PT_LIST; ++r, b &= b - 1)
+				if (r >= r0) s_start[r - r0] = (uint16_t)(my0 + __ffsll((long long)b));
+		}
+		__syncthreads();
+		const uint32_t cnt = n - r0 < PT_LIST ? n - r0 : PT_LIST;
+		for (uint32_t j0 = 0; j0 < cnt; j0 += PT_THREADS) {
+			const uint32_t j = j0 + threadIdx.x;
+			const uint64_t i = first + r0 + j;
+			uint32_t sq = NOSLOT, st = 0;
+			if (j < cnt) {
+				const uint64_t s = b0 + s_start[j];
+				uint64_t eol = r0 + j + 1 < n ? b0 + s_start[j + 1] - 1 : last_eol;
+				const char *base = eol <= w_end ? s_text - b0 : text; // base + window offset = address of that byte
+				if (eol - s > 1 && base[eol - 1] == '\r') --eol;
+				PLine r;
+				parse_line(base + s, base + eol, r, &s_vals[threadIdx.x >> 5][0][lane]);
+				if (r.nf >= 10) {
+					++n_parsed;
+					if (PASS == 2 && r.nf >= 11) last11 = (i + 1) << 31 | (r.bl & 0x7fffffffu);
+					if (!(r.qe - r.qs < (uint32_t)min_span || r.te - r.ts < (uint32_t)min_span || (int)(r.ml_rev & 0x7fffffffu) < min_match)) {
+						++n_pass;
+						if (PASS == 1) {
+							sq = win_insert(tab, text, base + s, r.qnl, s, 2 * i, r.ql, ws);
+							st = win_insert(tab, text, base + s + r.tdelta, r.tnl, s + r.tdelta, 2 * i + 1, r.tl, ws);
+						} else {
+							sq = win_find(tab, base + s, r.qnl), st = win_find(tab, base + s + r.tdelta, r.tnl);
+							if (sq == NOSLOT || st == NOSLOT) ++n_bad;  // a name pass 1 did not see: the source delivered other bytes
+							else {
+								const uint32_t qid = tab.t.id[sq], tid = tab.t.id[st], ord = (uint32_t)(2 * i);
+								const uint32_t bl = r.nf >= 11 ? r.bl & 0x7fffffffu : win_prev_bl(text, s, ws[WS_BL_IN]);
+								uint32_t at = atomicAdd(&cur[qid], 1u);
+								if (at < bfirst[qid + 1] - bfirst[qid]) {
+									uint4 *o = reinterpret_cast<uint4*>(out + bfirst[qid] + at);
+									o[0] = make_uint4(r.qs, ord, r.qe, tid);
+									o[1] = make_uint4(r.ts, r.te, r.ml_rev, bl);
+									++n_emit;
+								} else ++n_bad;                            // more hits than pass 1 counted for the read
+								if (bi_dir && qid != tid) { // the same overlap seen from the target (hit.c:92-98)
+									at = atomicAdd(&cur[tid], 1u);
+									if (at < bfirst[tid + 1] - bfirst[tid]) {
+										uint4 *o = reinterpret_cast<uint4*>(out + bfirst[tid] + at);
+										o[0] = make_uint4(r.ts, ord + 1, r.te, qid);
+										o[1] = make_uint4(r.qs, r.qe, r.ml_rev, bl);
+										++n_emit;
+									} else ++n_bad;
+								}
+							}
+						}
+					}
+				}
+			}
+			if (PASS == 1) { // consecutive lines often share their query read: one add per distinct slot of the warp
+				const unsigned grp = __match_any_sync(0xffffffffu, sq);
+				if (sq != NOSLOT && lane == (uint32_t)__ffs(grp) - 1) atomicAdd(&tab.t.hits[sq], (uint32_t)__popc(grp));
+				if (sq != NOSLOT && bi_dir && st != sq) atomicAdd(&tab.t.hits[st], 1u);
+			}
+		}
+		__syncthreads(); // the list is rewritten by the next round
+	}
+	n_parsed = __reduce_add_sync(0xffffffffu, n_parsed), n_pass = __reduce_add_sync(0xffffffffu, n_pass);
+	if (PASS == 2) {
+		n_bad = __reduce_add_sync(0xffffffffu, n_bad), n_emit = __reduce_add_sync(0xffffffffu, n_emit);
+		#pragma unroll
+		for (int o = 16; o; o >>= 1) { const unsigned long long y = __shfl_xor_sync(0xffffffffu, last11, o); last11 = y > last11 ? y : last11; }
+	}
+	if (lane == 0) {
+		if (n_parsed) atomicAdd(ws + WS_PARSED, (unsigned long long)n_parsed);
+		if (n_pass) atomicAdd(ws + WS_STORED, (unsigned long long)n_pass);
+		if (n_bad) atomicAdd(ws + WS_BAD, (unsigned long long)n_bad);
+		if (n_emit) atomicAdd(ws + WS_EMITTED, (unsigned long long)n_emit);
+		if (last11) atomicMax(ws + WS_BL_OUT, last11);
+	}
+}
+
+// ids and per-read counts from the dictionary of pass 1 (k_dict_rank without a text to read back from: the witness is in the
+// name store and first carries the length column)
+__global__ void k_win_rank(const unsigned long long *first_sorted, const uint64_t *slot_sorted, uint32_t n, WinTab t, uint64_t *noff, uint32_t *nlen, uint32_t *slen,
+                           unsigned long long *tot_len, uint32_t *read_cnt)
+{
+	unsigned long long sum = 0;
+	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+		const uint64_t s = slot_sorted[i], off = (t.t.key[s] & NT_OFF_MASK) - 1;
+		t.t.id[s] = i;
+		read_cnt[i] = t.t.hits[s];
+		uint32_t l = 0;
+		while (t.store[off + l] != '\t') ++l;
+		noff[i] = off, nlen[i] = l, slen[i] = (uint32_t)first_sorted[i]; // the length kept for a read is the one of its first appearance (sdict.c:36)
+		sum += slen[i];
+	}
+	typedef cub::BlockReduce<unsigned long long, 256> BR;
+	__shared__ typename BR::TempStorage ts;
+	unsigned long long s = BR(ts).Sum(sum);
+	if (threadIdx.x == 0 && s) atomicAdd(tot_len, s);
+}
+
+// The two windows on both sides of PCIe and what a launch over one of them needs.
+struct WinRun {
+	MabDev &d;
+	const TextSource &src;
+	size_t cap;                                              // bytes of a window
+	char *host[2] = {nullptr, nullptr}, *dev[2] = {nullptr, nullptr};
+	cudaEvent_t copied[2], parsed[2];                        // window k & 1: its bytes have landed / its launch is done
+	void *ts_mem = nullptr;
+	LineTileState ts;
+	unsigned *ctr = nullptr;
+	unsigned long long *ws = nullptr;
+
+	WinRun(MabDev &dev_, const TextSource &s, size_t w) : d(dev_), src(s), cap(0)
+	{
+		for (int i = 0; i < 2; ++i) {
+			MAB_CUDA(cudaEventCreateWithFlags(&copied[i], cudaEventDisableTiming));
+			MAB_CUDA(cudaEventCreateWithFlags(&parsed[i], cudaEventDisableTiming));
+		}
+		ctr = mab_alloc<unsigned>(d, 1);
+		ws = (unsigned long long*)mab_alloc<uint64_t>(d, WS_N);
+		if (!d.copy_stream) MAB_CUDA(cudaStreamCreateWithFlags(&d.copy_stream, cudaStreamNonBlocking));
+		resize(w, 0, 0);
+	}
+	~WinRun()
+	{
+		d.sync();
+		MAB_CUDA(cudaStreamSynchronize(d.copy_stream));
+		for (int i = 0; i < 2; ++i) {
+			MAB_CUDA(cudaFreeHost(host[i]));
+			d.free(dev[i]);
+			MAB_CUDA(cudaEventDestroy(copied[i])); MAB_CUDA(cudaEventDestroy(parsed[i]));
+		}
+		d.free(ts_mem); d.free(ctr); d.free(ws);
+	}
+	// windows of w bytes, keeping the first `keep` bytes of host window b (nothing is in flight when it is called with cap != 0)
+	void resize(size_t w, int b, size_t keep)
+	{
+		if (cap) { d.sync(); MAB_CUDA(cudaStreamSynchronize(d.copy_stream)); }
+		for (int i = 0; i < 2; ++i) {
+			char *nh;
+			MAB_CUDA(cudaMallocHost(&nh, w));
+			if (i == b && keep) memcpy(nh, host[i], keep);
+			if (host[i]) MAB_CUDA(cudaFreeHost(host[i]));
+			host[i] = nh;
+			if (dev[i]) d.free(dev[i]);
+			dev[i] = (char*)d.alloc(w + 64);                      // (+64: the tiles are staged in whole 16-byte words)
+		}
+		if (ts_mem) d.free(ts_mem);
+		ts = tiles_alloc(d, w / PT_TILE + 1, &ts_mem);
+		cap = w;
+	}
+};
+
+// One pass over the source: false when it cannot be rewound.  *n_bytes = bytes delivered.
+template <int PASS>
+static bool win_pass(WinRun &w, int min_span, int min_match, int bi_dir, const WinTab &tab, const uint32_t *bfirst, uint32_t *cur, DHit *out, uint64_t *n_bytes)
+{
+	MabDev &d = w.d;
+	if (w.src.rewind(w.src.ud) != 0) return false;
+	if (tab.store_cap + w.cap >= (1ull << NT_OFF_BITS) - 1) { fprintf(stderr, "[E::miniasm_b200] more than 2^37 bytes of read names and window\n"); exit(73); }
+	MAB_CUDA(cudaMemsetAsync(w.ws, 0, WS_N * 8, d.stream));
+	cudaEvent_t ready;
+	MAB_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
+	MAB_CUDA(cudaEventRecord(ready, d.stream));                 // the copies may not overtake whatever still uses the windows' memory on the main stream
+	MAB_CUDA(cudaStreamWaitEvent(d.copy_stream, ready, 0));
+	const char *tail = nullptr;                                 // the unfinished line after the previous window, still in its host buffer
+	size_t n_tail = 0, total = 0;
+	bool eof = false;
+	for (int b = 0; !eof; b ^= 1) {
+		MAB_CUDA(cudaEventSynchronize(w.copied[b]));            // the window that last used this host buffer has crossed
+		if (n_tail) memcpy(w.host[b], tail, n_tail);
+		size_t have = n_tail, cut = 0;
+		for (;;) {
+			while (have < w.cap) {
+				const size_t r = w.src.read(w.src.ud, w.host[b] + have, w.cap - have);
+				if (r == 0) { eof = true; break; }
+				have += r, total += r;
+			}
+			if (eof) { cut = have; break; }
+			const char *nl = (const char*)memrchr(w.host[b], '\n', have);
+			if (nl) { cut = (size_t)(nl - w.host[b]) + 1; break; }
+			w.resize(2 * w.cap, b, have);                       // a line longer than the window: the windows grow
+			if (tab.store_cap + w.cap >= (1ull << NT_OFF_BITS) - 1) { fprintf(stderr, "[E::miniasm_b200] more than 2^37 bytes of read names and window\n"); exit(73); }
+		}
+		tail = w.host[b] + cut, n_tail = have - cut;
+		if (cut == 0) break;                                    // (the end of the source, nothing left)
+		MAB_CUDA(cudaStreamWaitEvent(d.copy_stream, w.parsed[b], 0)); // the launch that last read this device window is done
+		MAB_CUDA(cudaMemcpyAsync(w.dev[b], w.host[b], cut, cudaMemcpyHostToDevice, d.copy_stream));
+		MAB_CUDA(cudaEventRecord(w.copied[b], d.copy_stream));
+		MAB_CUDA(cudaStreamWaitEvent(d.stream, w.copied[b], 0));
+		const uint64_t n_tile = (cut + PT_TILE - 1) / PT_TILE;
+		tiles_reset(d, w.ts, n_tile);
+		MAB_CUDA(cudaMemsetAsync(w.ctr, 0, 4, d.stream));
+		MAB_LAUNCH(d, k_win_tiles<PASS>, (unsigned)n_tile, PT_THREADS, 0, w.dev[b], cut, w.ctr, w.ts, min_span, min_match, bi_dir, tab, bfirst, cur, out, w.ws);
+		MAB_CUDA(cudaMemcpyAsync(w.ws + WS_LINE_IN, w.ws + WS_LINE_OUT, 16, cudaMemcpyDeviceToDevice, d.stream));
+		MAB_CUDA(cudaEventRecord(w.parsed[b], d.stream));
+	}
+	d.sync();
+	MAB_CUDA(cudaEventDestroy(ready));
+	*n_bytes = total;
+	return true;
+}
+
+bool ingest_paf_windowed(MabDev &d, const TextSource &src, size_t window_bytes, size_t size_hint, int min_span, int min_match, int bi_dir,
+                         DHits &h, DNames &names, char **name_text_out, IngestStats &st)
+{
+	memset(&st, 0, sizeof(st));
+	names = DNames();
+	h.n = 0, h.n_seq = 0;
+	*name_text_out = nullptr;
+	d.trace("ingest:begin");
+	if (window_bytes < (64u << 10)) window_bytes = 64u << 10;
+	WinRun w(d, src, (window_bytes + PT_TILE - 1) / PT_TILE * PT_TILE);
+	// table and name store from the size of the input when it is known; either one overflowing runs pass 1 again with four times the room
+	uint64_t cap = tab_cap_for(line_estimate(size_hint)), store_cap = size_hint / 32 > (8u << 20) ? size_hint / 32 : (8u << 20);
+	unsigned long long ws[WS_N];
+	uint64_t n_bytes = 0;
+	WinTab tab;
+	for (;;) {
+		tab.t = tab_alloc(d, cap, true);
+		tab.store = (char*)d.alloc(store_cap), tab.store_cap = store_cap;
+		const bool ok = win_pass<1>(w, min_span, min_match, bi_dir, tab, nullptr, nullptr, nullptr, &n_bytes);
+		if (ok) { MAB_CUDA(cudaMemcpyAsync(ws, w.ws, sizeof(ws), cudaMemcpyDeviceToHost, d.stream)); d.sync(); }
+		if (ok && !ws[WS_TAB_FULL] && !ws[WS_STORE_FULL]) break;
+		tab_free(d, tab.t); d.free(tab.store);
+		if (!ok) return false;
+		if (ws[WS_TAB_FULL]) cap <<= 2;
+		if (ws[WS_STORE_FULL]) store_cap <<= 2;
+		if (cap > (1ull << 32)) { fprintf(stderr, "[E::miniasm_b200] read-name table overflow\n"); exit(77); }
+	}
+	const uint64_t n_lines = ws[WS_LINE_IN];
+	st.n_lines = n_lines, st.n_parsed = ws[WS_PARSED];
+	const uint64_t n_stored = ws[WS_STORED];
+	if (2 * n_lines >= (1ull << 32)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 PAF lines on one GPU\n"); exit(73); }
+	d.trace("ingest:windowed pass 1 (parse + dictionary + hit counts)");
+	if (n_bytes == 0) { // (as ingest_paf leaves an empty text)
+		tab_free(d, tab.t); d.free(tab.store);
+		dh_reserve(d, h, 1);
+		return true;
+	}
+	// ids = rank of the first occurrence; the hit counts of the slots become those of the reads
+	uint64_t *slots = mab_alloc<uint64_t>(d, cap);
+	uint32_t n_seq;
+	{
+		cub::CountingInputIterator<uint64_t> pos(0);
+		SlotUsed used{tab.t.first};
+		size_t tb = 0;
+		unsigned long long *d_n = d.d_scal + SC_NSEL;
+		cub::DeviceSelect::If(nullptr, tb, pos, slots, d_n, (int64_t)cap, used, d.stream);
+		void *tmp = d.tmp(tb);
+		cub::DeviceSelect::If(tmp, tb, pos, slots, d_n, (int64_t)cap, used, d.stream);
+		++d.n_lib;
+		const uint64_t n = d.get_scal(SC_NSEL);
+		if (n >= (1ull << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 reads\n"); exit(73); }
+		n_seq = (uint32_t)n;
+	}
+	names.n_seq = n_seq;
+	names.off = mab_alloc<uint64_t>(d, n_seq); names.nlen = mab_alloc<uint32_t>(d, n_seq); names.slen = mab_alloc<uint32_t>(d, n_seq);
+	uint32_t *read_cnt = mab_alloc<uint32_t>(d, (size_t)n_seq + 1), *first = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);
+	MAB_CUDA(cudaMemsetAsync(read_cnt + n_seq, 0, 4, d.stream));
+	if (n_seq) {
+		unsigned long long *fa = (unsigned long long*)mab_alloc<uint64_t>(d, n_seq), *fb = (unsigned long long*)mab_alloc<uint64_t>(d, n_seq);
+		uint64_t *sb = mab_alloc<uint64_t>(d, n_seq);
+		MAB_LAUNCH(d, k_dict_pairs, mab_grid(n_seq, 256), 256, 0, slots, n_seq, tab.t, fa);
+		cub::DoubleBuffer<unsigned long long> dk(fa, fb);
+		cub::DoubleBuffer<uint64_t> dv(slots, sb);
+		size_t tb = 0;
+		cub::DeviceRadixSort::SortPairs(nullptr, tb, dk, dv, (int)n_seq, 32, 64, d.stream);   // by the occurrence number, the high half
+		void *tmp = d.tmp(tb);
+		cub::DeviceRadixSort::SortPairs(tmp, tb, dk, dv, (int)n_seq, 32, 64, d.stream);
+		++d.n_lib;
+		d.zero_scal(SC_AUX, 1);
+		MAB_LAUNCH(d, k_win_rank, mab_grid(n_seq, 256), 256, 0, dk.Current(), dv.Current(), n_seq, tab, names.off, names.nlen, names.slen, d.d_scal + SC_AUX, read_cnt);
+		st.tot_len = d.get_scal(SC_AUX);
+		d.free(fa); d.free(fb); d.free(sb);
+	}
+	d.free(slots);
+	d.trace("ingest:rank_ids");
+	dh_bucket_first(d, read_cnt, n_seq, first);
+	MAB_CUDA(cudaMemsetAsync(read_cnt, 0, (size_t)n_seq * 4, d.stream)); // the counts become the buckets' fill cursors
+	uint32_t n_hits;
+	MAB_CUDA(cudaMemcpyAsync(&n_hits, first + n_seq, 4, cudaMemcpyDeviceToHost, d.stream));
+	d.sync();
+	dh_reserve(d, h, n_hits ? n_hits : 1);
+	h.n = n_hits, h.n_seq = n_seq;
+	st.n_hits = n_hits, st.n_seq = n_seq;
+	// pass 2: every hit straight into its read's bucket of h.a2
+	uint64_t n_bytes2 = 0;
+	const bool ok2 = win_pass<2>(w, min_span, min_match, bi_dir, tab, first, read_cnt, h.a2, &n_bytes2);
+	if (ok2) { MAB_CUDA(cudaMemcpyAsync(ws, w.ws, sizeof(ws), cudaMemcpyDeviceToHost, d.stream)); d.sync(); }
+	tab_free(d, tab.t);
+	if (!ok2) {
+		d.free(tab.store); d.free(read_cnt); d.free(first);
+		names_free(d, names);
+		h.n = 0, h.n_seq = 0;
+		return false;
+	}
+	if (n_bytes2 != n_bytes || ws[WS_LINE_IN] != n_lines || ws[WS_PARSED] != st.n_parsed || ws[WS_STORED] != n_stored || ws[WS_BAD] || ws[WS_EMITTED] != n_hits) {
+		fprintf(stderr, "[E::miniasm_b200] the PAF source delivered a different text after rewinding: %llu bytes, %llu lines, %llu hits first, "
+		        "%llu bytes, %llu lines, %llu hits (%llu without a bucket) then\n", (unsigned long long)n_bytes, (unsigned long long)n_lines, (unsigned long long)n_hits,
+		        (unsigned long long)n_bytes2, ws[WS_LINE_IN], ws[WS_EMITTED], ws[WS_BAD]);
+		exit(78);
+	}
+	*name_text_out = tab.store;   // names.off points into it (owned by the caller from now on)
+	d.trace("ingest:windowed pass 2 (parse + emit_hits)");
+	dh_sort_buckets(d, h, first);
+	d.free(read_cnt); d.free(first);
+	d.trace("ingest:sort_hits");
+	return true;
+}

@@ -25,6 +25,14 @@ void ingest_paf(MabDev &d, const char *d_text, size_t len, int min_span, int min
 // load + ingest overlapped: host_text -> d_text in chunks on MabDev::copy_stream while arrived chunks are scanned and parsed
 void ingest_paf_stream(MabDev &d, char *d_text, const char *host_text, size_t len, int min_span, int min_match, int bi_dir,
                        DHits &h, DNames &names, IngestStats &st);
+// Windowed ingest: the text is delivered in order by `src` (read: the next bytes, 0 at the end; rewind: back to byte 0, nonzero
+// if impossible) and read twice, window_bytes (>= 64 KB, grown to the longest line) at a time; the device holds two windows, the
+// dictionary, a packed name store and the hits, never the text.  Same hits, names (names.off indexes *name_text_out, which the
+// caller frees) and counters as ingest_paf.  size_hint: bytes of the text when known (sizes the dictionary), else 0.
+// false: the source could not be rewound and nothing was ingested.  A source whose second delivery differs exits with code 78.
+struct TextSource { size_t (*read)(void *ud, char *dst, size_t cap); int (*rewind)(void *ud); void *ud; };
+bool ingest_paf_windowed(MabDev &d, const TextSource &src, size_t window_bytes, size_t size_hint, int min_span, int min_match, int bi_dir,
+                         DHits &h, DNames &names, char **name_text_out, IngestStats &st);
 void names_free(MabDev &d, DNames &n);
 // byte offsets of the line starts of a text in device memory (len > 0); free with d.free.  start[n_lines] is not set.
 uint64_t *dev_line_starts(MabDev &d, const char *d_text, size_t len, uint64_t *n_lines_out);
