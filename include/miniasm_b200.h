@@ -151,6 +151,11 @@ typedef struct {
 	double   ms_del_trans_kernel;                       /* CUDA-event time of the transitive-reduction kernel */
 	uint64_t n_kernel_launches, n_lib_calls;
 	double   ms_ingest, ms_select, ms_layout, ms_unitigs; /* CUDA-event time of the last call of each step */
+	uint64_t n_name_regrow;                             /* last ingest: read-name tables built again, not only for a full
+	                                                       dictionary: resident parse regrown (probe limit), windowed pass 1 rerun
+	                                                       (dictionary or name store full), streamed parse redone resident (full
+	                                                       dictionary, more lines than estimated, line cut at a chunk), sharded
+	                                                       global table re-seeded */
 } mab_stats_t;
 
 mab_ctx_t *mab_create(int device);                      /* exits if the device cannot be initialised */

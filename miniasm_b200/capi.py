@@ -128,7 +128,8 @@ class MabStats(C.Structure):                                          # mab_stat
     _fields_ = [(n, C.c_uint64) for n in ("n_lines", "n_hits_stored", "n_seq_in", "n_hits_final", "n_seq_final", "n_arc_sg",
                                           "n_arc_trans_in", "n_reduced", "trans_inner", "n_arc_final", "n_utg")] + \
                [("ms_del_trans_kernel", C.c_double), ("n_kernel_launches", C.c_uint64), ("n_lib_calls", C.c_uint64)] + \
-               [(n, C.c_double) for n in ("ms_ingest", "ms_select", "ms_layout", "ms_unitigs")]
+               [(n, C.c_double) for n in ("ms_ingest", "ms_select", "ms_layout", "ms_unitigs")] + \
+               [("n_name_regrow", C.c_uint64)]
 
 
 MAB_READ_FN = C.CFUNCTYPE(C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t)   # mab_text_source_t::read

@@ -387,7 +387,7 @@ int mab_ingest(mab_ctx_t *c, int min_span, int min_match, int bi_dir)
 	ctx_reset_reads(c);
 	ingest_paf(d, c->d_text, c->text_len, min_span, min_match, bi_dir, c->hits, c->names, c->ist);
 	c->n_seq = c->names.n_seq;
-	c->stats.n_lines = c->ist.n_parsed, c->stats.n_hits_stored = c->ist.n_hits, c->stats.n_seq_in = c->ist.n_seq;
+	c->stats.n_lines = c->ist.n_parsed, c->stats.n_hits_stored = c->ist.n_hits, c->stats.n_seq_in = c->ist.n_seq, c->stats.n_name_regrow = c->ist.name_regrow;
 	if (!mab_mute && ma_verbose >= 3)
 		fprintf(stderr, "[M::%s::%s] read %ld hits; stored %ld hits and %d sequences (%ld bp)\n", "ma_hit_read", sys_timestamp(),
 				(long)c->ist.n_parsed, (long)c->ist.n_hits, (int)c->ist.n_seq, (long)c->ist.tot_len);
@@ -407,7 +407,7 @@ int mab_load_ingest_text(mab_ctx_t *c, const char *text, size_t len, int min_spa
 	PhaseTimer pt(d, &c->stats.ms_ingest, "mab_load_ingest_text");
 	ingest_paf_stream(d, c->d_text, text, len, min_span, min_match, bi_dir, c->hits, c->names, c->ist);
 	c->n_seq = c->names.n_seq;
-	c->stats.n_lines = c->ist.n_parsed, c->stats.n_hits_stored = c->ist.n_hits, c->stats.n_seq_in = c->ist.n_seq;
+	c->stats.n_lines = c->ist.n_parsed, c->stats.n_hits_stored = c->ist.n_hits, c->stats.n_seq_in = c->ist.n_seq, c->stats.n_name_regrow = c->ist.name_regrow;
 	if (!mab_mute && ma_verbose >= 3)
 		fprintf(stderr, "[M::%s::%s] read %ld hits; stored %ld hits and %d sequences (%ld bp)\n", "ma_hit_read", sys_timestamp(),
 				(long)c->ist.n_parsed, (long)c->ist.n_hits, (int)c->ist.n_seq, (long)c->ist.tot_len);
@@ -425,7 +425,7 @@ static int ingest_windowed(mab_ctx *c, const TextSource &src, size_t window_byte
 	if (!ingest_paf_windowed(d, src, window_bytes ? window_bytes : (size_t)256 << 20, size_hint, min_span, min_match, bi_dir, c->hits, c->names, &c->name_text, c->ist))
 		return -1;
 	c->n_seq = c->names.n_seq;
-	c->stats.n_lines = c->ist.n_parsed, c->stats.n_hits_stored = c->ist.n_hits, c->stats.n_seq_in = c->ist.n_seq;
+	c->stats.n_lines = c->ist.n_parsed, c->stats.n_hits_stored = c->ist.n_hits, c->stats.n_seq_in = c->ist.n_seq, c->stats.n_name_regrow = c->ist.name_regrow;
 	if (!mab_mute && ma_verbose >= 3)
 		fprintf(stderr, "[M::%s::%s] read %ld hits; stored %ld hits and %d sequences (%ld bp)\n", "ma_hit_read", sys_timestamp(),
 				(long)c->ist.n_parsed, (long)c->ist.n_hits, (int)c->ist.n_seq, (long)c->ist.tot_len);
@@ -500,7 +500,7 @@ int mab_ingest_nocont(mab_ctx_t *c, int min_span, int min_match, int bi_dir, int
 	NoContParams nc = { max_hang, int_frac };
 	ingest_paf(d, c->d_text, c->text_len, min_span, min_match, bi_dir, c->hits, c->names, c->ist, &nc);
 	c->n_seq = c->names.n_seq;
-	c->stats.n_lines = c->ist.n_parsed, c->stats.n_hits_stored = c->ist.n_hits, c->stats.n_seq_in = c->ist.n_seq;
+	c->stats.n_lines = c->ist.n_parsed, c->stats.n_hits_stored = c->ist.n_hits, c->stats.n_seq_in = c->ist.n_seq, c->stats.n_name_regrow = c->ist.name_regrow;
 	if (!mab_mute && ma_verbose >= 3) fprintf(stderr, "[M::%s::%s] dropped %d contained reads\n", "ma_hit_no_cont", sys_timestamp(), (int)c->ist.n_dropped);
 	if (!mab_mute) fprintf(stderr, "[M::main] ===> Step 1: reading read mappings <===\n");
 	if (!mab_mute && ma_verbose >= 3)
@@ -545,7 +545,7 @@ int mab_load_hits(mab_ctx_t *c, const ma_hit_t *a, size_t n, const sdict_t *dict
 	d.sync();
 	free(pack); free(off); free(nl); free(sl);
 	c->n_seq = dict->n_seq;
-	c->stats.n_hits_stored = n, c->stats.n_seq_in = dict->n_seq;
+	c->stats.n_hits_stored = n, c->stats.n_seq_in = dict->n_seq, c->stats.n_name_regrow = 0;
 	return 0;
 }
 
@@ -1026,7 +1026,7 @@ int mab_ingest_sharded(mab_ctx_t *c, int min_span, int min_match, int bi_dir)
 	ctx_reset_reads(c);
 	ingest_paf_sharded(d, c->sc, c->d_text, c->text_len, min_span, min_match, bi_dir, c->hits, c->names, &c->name_text, c->ist);
 	c->n_seq = c->names.n_seq;
-	c->stats.n_lines = c->ist.n_parsed, c->stats.n_hits_stored = c->ist.n_hits, c->stats.n_seq_in = c->ist.n_seq;
+	c->stats.n_lines = c->ist.n_parsed, c->stats.n_hits_stored = c->ist.n_hits, c->stats.n_seq_in = c->ist.n_seq, c->stats.n_name_regrow = c->ist.name_regrow;
 	if (!mab_mute && ma_verbose >= 3 && c->sc.rank == 0)
 		fprintf(stderr, "[M::%s::%s] read %ld hits; stored %ld hits and %d sequences (%ld bp)\n", "ma_hit_read", sys_timestamp(),
 				(long)c->ist.n_parsed, (long)c->ist.n_hits, (int)c->ist.n_seq, (long)c->ist.tot_len);
@@ -1044,7 +1044,7 @@ int mab_load_ingest_text_sharded(mab_ctx_t *c, const char *text, size_t len, int
 	PhaseTimer pt(d, &c->stats.ms_ingest, "mab_load_ingest_text_sharded");
 	ingest_paf_sharded(d, c->sc, c->d_text, c->text_len, min_span, min_match, bi_dir, c->hits, c->names, &c->name_text, c->ist, text);
 	c->n_seq = c->names.n_seq;
-	c->stats.n_lines = c->ist.n_parsed, c->stats.n_hits_stored = c->ist.n_hits, c->stats.n_seq_in = c->ist.n_seq;
+	c->stats.n_lines = c->ist.n_parsed, c->stats.n_hits_stored = c->ist.n_hits, c->stats.n_seq_in = c->ist.n_seq, c->stats.n_name_regrow = c->ist.name_regrow;
 	if (!mab_mute && ma_verbose >= 3 && c->sc.rank == 0)
 		fprintf(stderr, "[M::%s::%s] read %ld hits; stored %ld hits and %d sequences (%ld bp)\n", "ma_hit_read", sys_timestamp(),
 				(long)c->ist.n_parsed, (long)c->ist.n_hits, (int)c->ist.n_seq, (long)c->ist.tot_len);

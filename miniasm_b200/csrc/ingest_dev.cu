@@ -581,6 +581,7 @@ struct Parsed {
 	PRec *ln = nullptr;
 	NameTab tab{nullptr, nullptr, nullptr, 0};
 	uint64_t cap = 0, n_lines = 0, n_parsed = 0;
+	uint32_t regrow = 0;         // dictionary overflows that made the parse run again with a larger table
 };
 
 // Room for the lines before they are counted (a PAF line of 12 columns has at least 24 bytes) and the dictionary size
@@ -631,7 +632,7 @@ static void parse_resident(MabDev &d, const char *d_text, size_t len, int min_sp
 		if (!more_lines && !overflow) break;
 		d.free(p.start); d.free(p.ln); tab_free(d, p.tab);
 		if (more_lines) line_cap = p.n_lines;
-		if (overflow) cap <<= 2;
+		if (overflow) cap <<= 2, ++p.regrow;
 		if (cap > (1ull << 33)) { fprintf(stderr, "[E::miniasm_b200] read-name table overflow\n"); exit(77); }
 	}
 	d.free(ctr); d.free(ts_mem);
@@ -654,7 +655,7 @@ void ingest_paf(MabDev &d, const char *d_text, size_t len, int min_span, int min
 	// (1)+(2) line starts, parse, store filter, dictionary insert and hit counts per name in one pass
 	Parsed p;
 	parse_resident(d, d_text, len, min_span, min_match, bi_dir, true, p);
-	st.n_parsed = p.n_parsed, st.n_lines = p.n_lines;
+	st.n_parsed = p.n_parsed, st.n_lines = p.n_lines, st.name_regrow = p.regrow;
 	d.trace("ingest:parse");
 	ingest_finish(d, d_text, len, p.start, p.ln, p.n_lines, p.tab, p.cap, bi_dir, nocont, h, names, st);
 }
@@ -726,6 +727,7 @@ void ingest_paf_stream(MabDev &d, char *d_text, const char *host_text, size_t le
 	Parsed p;
 	if (!stream_parse(d, d_text, host_text, len, min_span, min_match, bi_dir, true, p)) {
 		ingest_paf(d, d_text, len, min_span, min_match, bi_dir, h, names, st, nullptr); // the text is resident now: the plain path parses it again
+		++st.name_regrow;
 		return;
 	}
 	st.n_parsed = p.n_parsed, st.n_lines = p.n_lines;
@@ -889,15 +891,19 @@ __global__ void k_gtab_insert(const GEntry *ent, uint64_t n, GTab t, uint32_t *s
 	}
 }
 
+// an entry that found no slot (slot_of = 0xffffffff, counted by k_gtab_insert) is skipped: the table is built again with another seed
 __global__ void k_gtab_winner(const GEntry *ent, uint64_t n, GTab t, const uint32_t *slot_of)
 {
-	for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
-		if (t.first[slot_of[i]] == ent[i].first) t.win[slot_of[i]] = (uint32_t)i; // first occurrences are unique: exactly one winner
+	for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+		const uint32_t s = slot_of[i];
+		if (s != 0xffffffffu && t.first[s] == ent[i].first) t.win[s] = (uint32_t)i; // first occurrences are unique: exactly one winner
+	}
 }
 
 __global__ void k_gtab_verify(const GEntry *ent, uint64_t n, GTab t, const uint32_t *slot_of, const uint64_t *name_pos, const char *names, unsigned long long *n_bad)
 {
 	for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+		if (slot_of[i] == 0xffffffffu) continue;                         // (no slot: already an overflow, the table is redone)
 		const uint32_t w = t.win[slot_of[i]];
 		if (w == i) continue;
 		bool ok = ent[w].nlen == ent[i].nlen;
@@ -1096,6 +1102,7 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 		d.trace("shard-ingest:stream (copy + parse + dictionary)");
 	}
 	if (!have) parse_resident(d, d_text, len, min_span, min_match, bi_dir, false, p); // (local: the dictionary grows on this rank alone)
+	st.name_regrow = p.regrow + (host_text && len && !have ? 1 : 0);
 	uint64_t *start = p.start, n_lines = p.n_lines, cap = p.cap, n_parsed = p.n_parsed;
 	PRec *ln = p.ln;
 	NameTab tab = p.tab;
@@ -1200,7 +1207,7 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 		d.free(gt.key); d.free(gt.first); d.free(gt.win); d.free(gt.id);
 		d.free(g_ent); d.free(g_names); d.free(g_pos);
 		seed = seed * 6364136223846793005ULL + 1442695040888963407ULL;
-		++st.hash_retries;
+		++st.hash_retries, ++st.name_regrow;
 		if (attempt > 16) { fprintf(stderr, "[E::miniasm_b200] read-name hashing keeps colliding\n"); exit(77); }
 	}
 	d.trace("shard-ingest:global table");
@@ -1751,6 +1758,7 @@ bool ingest_paf_windowed(MabDev &d, const TextSource &src, size_t window_bytes, 
 		if (!ok) return false;
 		if (ws[WS_TAB_FULL]) cap <<= 2;
 		if (ws[WS_STORE_FULL]) store_cap <<= 2;
+		++st.name_regrow;
 		if (cap > (1ull << 32)) { fprintf(stderr, "[E::miniasm_b200] read-name table overflow\n"); exit(77); }
 	}
 	const uint64_t n_lines = ws[WS_LINE_IN];

@@ -13,7 +13,11 @@ struct DNames {
 	uint32_t *slen = nullptr;    // sequence length recorded at first appearance
 };
 
-struct IngestStats { uint64_t n_lines, n_parsed, n_hits, n_seq, tot_len, n_dropped; int hash_retries; };
+// name_regrow: how often the ingest built its read-name table again.  Not only dictionary overflows: it counts the resident parse
+// regrown after a probe run hit its limit; every rerun of windowed pass 1, whether the dictionary or only the name store was full;
+// every streamed parse given up for the resident one, whether for a full dictionary, more lines than estimated or a line cut at a
+// chunk; and every re-seed of the sharded global table (hash_retries of them)
+struct IngestStats { uint64_t n_lines, n_parsed, n_hits, n_seq, tot_len, n_dropped; int hash_retries; uint32_t name_regrow; };
 struct NoContParams { int max_hang; float int_frac; }; // -R (ma_hit_no_cont, hit.c:38-68)
 
 // d_text: the PAF bytes in device memory.  On return `h` holds the sorted hits (ma_hit_sort order, stable) and

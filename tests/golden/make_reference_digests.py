@@ -14,7 +14,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 TESTS = ["tests/test_asg_gpu.py", "tests/test_clean_gpu.py", "tests/test_hit_gpu.py", "tests/test_cli_gpu.py", "tests/test_switches_gpu.py",
-         "tests/test_shard_gpu.py", "tests/test_oracle_cpu.py", "tests/test_abi_cpu.py::test_struct_layouts_match_ctypes_and_reference"]
+         "tests/test_shard_gpu.py", "tests/test_oracle_cpu.py", "tests/test_name_collisions_gpu.py", "tests/test_abi_cpu.py::test_struct_layouts_match_ctypes_and_reference"]
 # tests of the CUDA library alone: nothing of the reference to record
 PRODUCT_ONLY = ["tests/test_hit_gpu.py::test_streamed_ingest_equals_two_calls", "tests/test_asg_gpu.py::test_empty_graph",
                 "tests/test_hit_gpu.py::test_empty_inputs"]

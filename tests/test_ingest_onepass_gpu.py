@@ -165,7 +165,7 @@ def oracle(port, path, nocont):
     return canon(hits), names
 
 
-def ours(prod, data, route):
+def ours(prod, data, route, regrow=None):
     opt = prod.default_opt()
     ctx = prod.mab_create(0)
     if route.startswith("shard"):
@@ -191,11 +191,13 @@ def ours(prod, data, route):
     prod.sd_destroy(d)
     st = prod.mab_stats(ctx).contents
     counters = (st.n_lines, st.n_hits_stored, st.n_seq_in)
+    if regrow is not None:                  # how often the ingest built a read-name table again
+        regrow[route] = st.n_name_regrow
     prod.mab_destroy(ctx)
     return canon(hits), names, counters
 
 
-def check(prod, port, data, path, routes=ROUTES):
+def check(prod, port, data, path, routes=ROUTES, regrow=None):
     with open(path, "wb") as f:
         f.write(data)
     want = {False: oracle(port, path, False)}
@@ -205,7 +207,7 @@ def check(prod, port, data, path, routes=ROUTES):
         if nocont not in want:
             want[nocont] = oracle(port, path, True)
         w_hits, w_names = want[nocont]
-        hits, names, counters = ours(prod, data, route)
+        hits, names, counters = ours(prod, data, route, regrow)
         assert names == w_names, f"{route}: read names / lengths differ"
         assert np.array_equal(hits, w_hits), f"{route}: hits differ ({len(hits)} vs {len(w_hits)})"
         assert counters == (n_parsed, len(w_hits), len(w_names)), f"{route}: counters {counters}"

@@ -79,24 +79,26 @@ def resident(prod, data):
     return out
 
 
-def windowed(prod, data, window, **kw):
+def windowed(prod, data, window, regrow=None, **kw):
     opt = prod.default_opt()
     ctx = prod.mab_create(0)
     src = Source(data, **kw)
     assert prod.mab_ingest_windowed(ctx, C.byref(src.struct), window, opt.min_span, opt.min_match, 1) == 0
     out = state(prod, ctx)
+    if regrow is not None:                  # how often pass 1 ran again with a larger dictionary or name store
+        regrow[window] = prod.mab_stats(ctx).contents.n_name_regrow
     prod.mab_destroy(ctx)
     return out, src
 
 
-def check(prod, port, data, path, windows=WINDOWS, **kw):
+def check(prod, port, data, path, windows=WINDOWS, regrow=None, **kw):
     with open(path, "wb") as f:
         f.write(data)
     w_hits, w_names = oracle(port, path, False)
     r_hits, r_names, r_counters = resident(prod, data)
     assert r_names == w_names and np.array_equal(canon(r_hits), w_hits)
     for window in windows:
-        (hits, names, counters), src = windowed(prod, data, window, **kw)
+        (hits, names, counters), src = windowed(prod, data, window, regrow, **kw)
         assert names == w_names, f"window {window}: read names / lengths differ"
         assert np.array_equal(canon(hits), w_hits), f"window {window}: hits differ ({len(hits)} vs {len(w_hits)})"
         assert counters == (parsed_lines(data), len(w_hits), len(w_names)) == r_counters, f"window {window}: counters {counters}"
