@@ -184,7 +184,8 @@ int mab_load_ingest_text(mab_ctx_t *ctx, const char *text, size_t len, int min_s
  * mab_ingest leaves (a text loaded before is dropped).  The source must deliver the same bytes after rewind: a difference
  * ends the process with exit code 78.  Returns 0; mab_ingest_windowed -1 when rewind fails (nothing ingested, the context stays
  * usable); mab_ingest_file_windowed -1 when the file cannot be opened and -2 when it cannot be rewound ("-" on a pipe).  A
- * gzip file is inflated by zlib on the host here, twice. */
+ * regular gzip file is inflated on the GPU a compressed segment at a time, straight into the device windows, once per pass
+ * (window_bytes = 0: 1 GB windows for gzip); a stream the GPU decoder rejects starts over through zlib on the host. */
 typedef struct {
 	size_t (*read)(void *ud, char *dst, size_t cap);  /* next bytes in order, 0 at the end */
 	int    (*rewind)(void *ud);                       /* back to byte 0; -1 if impossible */
@@ -192,6 +193,13 @@ typedef struct {
 } mab_text_source_t;
 int mab_ingest_windowed(mab_ctx_t *ctx, const mab_text_source_t *src, size_t window_bytes, int min_span, int min_match, int bi_dir);
 int mab_ingest_file_windowed(mab_ctx_t *ctx, const char *fn, size_t window_bytes, int min_span, int min_match, int bi_dir);
+/* The windowed counterpart of mab_load_paf_gz: gzip PAF held in host memory (gz[0, len), which must stay valid throughout),
+ * inflated on the GPU a segment at a time into the windows of mab_ingest_windowed, twice.  window_bytes bounds the inflated
+ * bytes per window (0: 1 GB; smaller windows inflate more slowly).  The decoder's scratch besides is S x (2 + 96 KiB / C) for
+ * segments of S compressed bytes (about 0.4 x window_bytes for PAF, at most window_bytes + 16 KiB) in chunks of C = 4-64 KiB:
+ * 3.5-5 S for windows of 1 GB and more, up to 26 S below about 160 MB (DESIGN.md 3c).  Returns 0, or -2 when the GPU
+ * decoder rejects the stream (nothing ingested, the context stays usable). */
+int mab_ingest_gz_windowed(mab_ctx_t *ctx, const void *gz, size_t len, size_t window_bytes, int min_span, int min_match, int bi_dir);
 /* high-water mark, in bytes, of the device memory the context's allocator handed out; reset != 0 restarts it at the current use */
 size_t mab_mem_peak(mab_ctx_t *ctx, int reset);
 /* device memory, in bytes, the context could still take: what the driver reports free plus what its allocator holds unused */

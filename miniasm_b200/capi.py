@@ -153,6 +153,7 @@ _PRODUCT_ONLY = {
     "mab_load_ingest_text": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int]),
     "mab_ingest_windowed": (C.c_int, [C.c_void_p, C.POINTER(MabTextSource), C.c_size_t, C.c_int, C.c_int, C.c_int]),
     "mab_ingest_file_windowed": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t, C.c_int, C.c_int, C.c_int]),
+    "mab_ingest_gz_windowed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.c_int]),
     "mab_mem_peak": (C.c_size_t, [C.c_void_p, C.c_int]),
     "mab_mem_free": (C.c_size_t, [C.c_void_p]),
     "mab_ingest_nocont": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),

@@ -238,8 +238,9 @@ static int gz_open_regular(const char *fn, size_t *size)
 	return -1;
 }
 
-// size bytes of fd to dst (device) through two pinned staging buffers of CH bytes: the read of chunk k+1 overlaps the copy of chunk k
-static bool read_to_dev(int fd, size_t size, char *dst, char *const pin[2], size_t CH, cudaStream_t st)
+// size bytes of fd from byte `at` to dst (device) through two pinned staging buffers of CH bytes: the read of chunk k+1 overlaps
+// the copy of chunk k
+static bool read_to_dev(int fd, size_t size, char *dst, char *const pin[2], size_t CH, cudaStream_t st, uint64_t at = 0)
 {
 	cudaEvent_t ev[2];
 	for (int i = 0; i < 2; ++i) MAB_CUDA(cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming));
@@ -250,7 +251,7 @@ static bool read_to_dev(int fd, size_t size, char *dst, char *const pin[2], size
 		const size_t want = size - done < CH ? size - done : CH;
 		size_t got = 0;
 		while (got < want) {
-			const ssize_t r = pread(fd, pin[k] + got, want - got, (off_t)(done + got));
+			const ssize_t r = pread(fd, pin[k] + got, want - got, (off_t)(at + done + got));
 			if (r <= 0) { ok = false; break; }
 			got += (size_t)r;
 		}
@@ -438,7 +439,7 @@ int mab_ingest_windowed(mab_ctx_t *c, const mab_text_source_t *src, size_t windo
 	return ingest_windowed(c, ts, window_bytes, 0, min_span, min_match, bi_dir);
 }
 
-struct FileSource { int fd; gzFile gz; }; // a plain file is read and sought directly, a gzip file through zlib on the host
+struct FileSource { int fd; gzFile gz; }; // a plain file is read and sought directly, a gzip file GPU rejects through zlib on the host
 
 static size_t file_read(void *ud, char *dst, size_t cap)
 {
@@ -455,6 +456,74 @@ static int file_rewind(void *ud)
 	return f->gz ? gzrewind(f->gz) : lseek(f->fd, 0, SEEK_SET) == 0 ? 0 : -1;
 }
 
+// ---- a gzip stream inflated on the GPU into the windows (GzStream, DESIGN.md 3c/3d) ---------------------------------------
+// window_bytes = 0 for a gzip source: the decode's parallelism is the number of units in a segment, and a segment takes about a
+// window of output, so the windows are larger than for text (DESIGN.md 3d: measured on config 3)
+static const size_t GZ_WINDOW_DEFAULT = (size_t)1 << 30;
+
+struct HostGzInput : GzInput { // compressed bytes in host memory
+	const uint8_t *p;
+	explicit HostGzInput(const void *q) : p((const uint8_t*)q) {}
+	bool read(uint64_t off, size_t n, uint8_t *d_dst, cudaStream_t st) override
+	{
+		MAB_CUDA(cudaMemcpyAsync(d_dst, p + off, n, cudaMemcpyHostToDevice, st));
+		return true;
+	}
+};
+
+struct FileGzInput : GzInput { // a regular file, read in segment-sized pieces through the context's pinned buffers
+	int fd;
+	mab_ctx *c;
+	FileGzInput(int f, mab_ctx *ctx) : fd(f), c(ctx) {}
+	bool read(uint64_t off, size_t n, uint8_t *d_dst, cudaStream_t st) override { return read_to_dev(fd, n, (char*)d_dst, c->pin, c->pin_bytes, st, off); }
+};
+
+struct GzSource { GzStream *gs; bool rejected; };
+
+static int64_t gz_fill(void *ud, char *d_dst, size_t cap)
+{
+	GzSource *g = (GzSource*)ud;
+	const int64_t r = g->gs->fill(d_dst, cap);
+	if (r == GZ_SMALL) return TS_FULL;
+	if (r < 0) { g->rejected = true; return TS_FAIL; }
+	return r;
+}
+
+static int gz_rewind(void *ud) { ((GzSource*)ud)->gs->rewind(); return 0; }
+
+// 0, or -2 when the GPU decoder rejected the stream in the first pass (nothing ingested)
+static int ingest_gz_windowed(mab_ctx *c, GzInput &in, uint64_t len, size_t window_bytes, int min_span, int min_match, int bi_dir, const char *what)
+{
+	MAB_CUDA(cudaSetDevice(c->dev.device));
+	const double t0 = sys_realtime();
+	const char *ch = getenv("MAB_GZ_CHUNK"); // (a measurement knob: compressed bytes per unit; unset = from the segment size)
+	int rc;
+	{
+		ArenaMem am(c->dev);
+		GzStream gs(c->dev.stream, am, in, len, ch ? (size_t)strtoull(ch, 0, 10) : 0);
+		GzSource src = { &gs, false };
+		const TextSource ts = { nullptr, gz_rewind, &src, gz_fill };
+		rc = ingest_windowed(c, ts, window_bytes ? window_bytes : GZ_WINDOW_DEFAULT, len * 4, min_span, min_match, bi_dir);
+		if (getenv("MAB_TRACE"))
+			fprintf(stderr, "[T::gzstream] %s: rc %d, %.3f ms; read %.3f find %.3f decode %.3f chain %.3f window %.3f resolve %.3f crc %.3f ms; "
+			        "%llu segments (%llu grown), %llu chunks, %llu units, %llu chained, %llu bytes out, scratch peak %llu\n", what,
+			        src.rejected ? -2 : rc, (sys_realtime() - t0) * 1e3, gs.ms_read, gs.sum.ms_find, gs.sum.ms_decode, gs.sum.ms_chain,
+			        gs.sum.ms_window, gs.sum.ms_resolve, gs.sum.ms_crc, (unsigned long long)gs.n_segments, (unsigned long long)gs.n_grown,
+			        (unsigned long long)gs.sum.n_chunks, (unsigned long long)gs.sum.n_units, (unsigned long long)gs.sum.n_chain,
+			        (unsigned long long)gs.sum.out_len, (unsigned long long)gs.sum.scratch_peak);
+		if (src.rejected) rc = -2;
+	}
+	return rc;
+}
+
+int mab_ingest_gz_windowed(mab_ctx_t *c, const void *gz, size_t len, size_t window_bytes, int min_span, int min_match, int bi_dir)
+{
+	MAB_CUDA(cudaSetDevice(c->dev.device));
+	if (!gz_magic(gz, len)) return -2;
+	HostGzInput in(gz);
+	return ingest_gz_windowed(c, in, len, window_bytes, min_span, min_match, bi_dir, "mab_ingest_gz_windowed") == 0 ? 0 : -2;
+}
+
 int mab_ingest_file_windowed(mab_ctx_t *c, const char *fn, size_t window_bytes, int min_span, int min_match, int bi_dir)
 {
 	FileSource f = { fn && strcmp(fn, "-") ? open(fn, O_RDONLY) : dup(fileno(stdin)), nullptr };
@@ -463,6 +532,11 @@ int mab_ingest_file_windowed(mab_ctx_t *c, const char *fn, size_t window_bytes, 
 	uint8_t mg[2];
 	size_t hint = fstat(f.fd, &sb) == 0 && S_ISREG(sb.st_mode) ? (size_t)sb.st_size : 0;
 	if (hint && pread(f.fd, mg, 2, 0) == 2 && gz_magic(mg, 2)) {
+		// a regular gzip file: inflated on the GPU a segment at a time; a stream the GPU decoder rejects starts over through zlib
+		MAB_CUDA(cudaSetDevice(c->dev.device));
+		pins_reserve(c, 64u << 20);
+		FileGzInput in(f.fd, c);
+		if (ingest_gz_windowed(c, in, hint, window_bytes, min_span, min_match, bi_dir, "mab_ingest_file_windowed") == 0) { close(f.fd); return 0; }
 		f.gz = gzdopen(f.fd, "r");
 		if (f.gz == 0) { close(f.fd); return -1; }
 		gzbuffer(f.gz, 1 << 20);

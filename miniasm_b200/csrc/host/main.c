@@ -138,20 +138,23 @@ static mab_ctx_t *run_sharded(const char *fn, const ma_opt_t *opt, int bi_dir, i
 	return ctx0;
 }
 
-/* MINIASM_B200_INGEST=auto: does Step 1 take the windowed ingest?  Only for a plain regular file whose text and line arrays
- * (what the resident ingest holds beside the hits: the padded text, a line start and a 32-byte record per estimated line) would
- * take more than half of the free device memory -- inputs the resident ingest cannot hold.  The half is a guess, not a measurement. */
+/* MINIASM_B200_INGEST=auto: does Step 1 take the windowed ingest?  Only for a regular file whose text and line arrays (what the
+ * resident ingest holds beside the hits: the padded text, a line start and a 32-byte record per estimated line) would take more
+ * than half of the free device memory -- inputs the resident ingest cannot hold.  The half is a guess, not a measurement.  For a
+ * gzip file the text's length is guessed as 4 x the compressed size (the guess mab_ingest_file_windowed sizes its dictionary by;
+ * PAF compresses about 3.6-fold with gzip -1), not read from the file. */
 static int auto_windowed(mab_ctx_t *ctx, const char *fn)
 {
 	struct stat sb;
 	unsigned char magic[2] = {0, 0};
-	int fd, plain;
+	int fd, regular, gz;
 	size_t len;
 	if (strcmp(fn, "-") == 0 || (fd = open(fn, O_RDONLY)) < 0) return 0;
-	plain = fstat(fd, &sb) == 0 && S_ISREG(sb.st_mode) && !(pread(fd, magic, 2, 0) == 2 && magic[0] == 0x1f && magic[1] == 0x8b);
+	regular = fstat(fd, &sb) == 0 && S_ISREG(sb.st_mode);
+	gz = regular && pread(fd, magic, 2, 0) == 2 && magic[0] == 0x1f && magic[1] == 0x8b;
 	close(fd);
-	if (!plain) return 0;
-	len = (size_t)sb.st_size;
+	if (!regular) return 0;
+	len = (size_t)sb.st_size * (gz ? 4 : 1);
 	return len / 8 * 9 + 40 * (len / 24 + 1024) > mab_mem_free(ctx) / 2;
 }
 

@@ -9,7 +9,8 @@
 //     unit's own first output byte is stored as a marker 256 + w, naming byte w of the 32 KiB window that precedes the unit.
 //   pass 2 (InfOutByte): the resolved window of the predecessor is known; bytes go straight to their final place.
 // Both passes stop at the first block boundary that lands exactly on a later unit's start (INF_LAND), or at the end of the
-// input right after a gzip trailer (INF_END).
+// input right after a gzip trailer (INF_END).  A fault found only after reading past the end of the input is INF_SHORT: with
+// the whole file that is truncation, with a piece of it (the streaming decoder of gzstream.cuh) it asks for more bytes.
 #pragma once
 #include <stdint.h>
 
@@ -21,7 +22,7 @@
 #define INF_HD_NOINL inline
 #endif
 
-enum { INF_END = 1, INF_LAND = 2, INF_ERR = -1 };
+enum { INF_END = 1, INF_LAND = 2, INF_ERR = -1, INF_SHORT = -2 };
 enum { INF_WIN = 32768, INF_WMASK = INF_WIN - 1 };
 #define INF_CRC_POLY 0xEDB88320u
 
@@ -256,29 +257,30 @@ INF_HD uint32_t inf_crc_final(const uint32_t *x2k, uint32_t raw, uint64_t n)
 	return ~(raw ^ inf_gf2_mul(0xffffffffu, inf_x8n(x2k, n)));
 }
 
-// ---- gzip member header (RFC 1952 2.3) at byte `at`: returns the byte offset of the deflate data, or -1 -------------------
+// ---- gzip member header (RFC 1952 2.3) at byte `at`: returns the byte offset of the deflate data, -1 for a bad header or -2
+// for one the input ends inside (every byte present so far is a valid header prefix)
 INF_HD int64_t inf_gzip_header(const uint8_t *p, uint64_t n, uint64_t at)
 {
 	uint64_t i = at;
-	if (n < 10 || at > n - 10) return -1;
-	if (p[i] != 0x1f || p[i + 1] != 0x8b || p[i + 2] != 8) return -1;
+	if (at >= n) return -2;
+	if (p[i] != 0x1f || (n - i > 1 && p[i + 1] != 0x8b) || (n - i > 2 && p[i + 2] != 8) || (n - i > 3 && (p[i + 3] & 0xe0))) return -1;
+	if (n < 10 || at > n - 10) return -2;
 	const uint8_t flg = p[i + 3];
-	if (flg & 0xe0) return -1;
 	i += 10;
 	if (flg & 4) { // FEXTRA
-		if (i + 2 > n) return -1;
+		if (i + 2 > n) return -2;
 		const uint64_t xlen = p[i] | (uint64_t)p[i + 1] << 8;
 		i += 2;
-		if (xlen > n - i) return -1;
+		if (xlen > n - i) return -2;
 		i += xlen;
 	}
 	for (int f = 8; f <= 16; f <<= 1) if (flg & f) { // FNAME, FCOMMENT: zero-terminated
 		while (i < n && p[i]) ++i;
-		if (i >= n) return -1;
+		if (i >= n) return -2;
 		++i;
 	}
 	if (flg & 2) { // FHCRC: the two low bytes of the CRC-32 of the header up to here
-		if (i + 2 > n) return -1;
+		if (i + 2 > n) return -2;
 		const uint32_t c = inf_crc_bitwise(0, p + at, i - at);
 		if ((c & 0xffff) != (uint32_t)(p[i] | p[i + 1] << 8)) return -1;
 		i += 2;
@@ -358,11 +360,12 @@ INF_HD_NOINL int inf_run(const uint8_t *gz, uint64_t n, uint64_t bit, bool at_he
 	in.init(gz, n, bit);
 	bool header = at_header, first = true;
 	t.kind = 0;
+#define INF_FAIL return in.over() ? INF_SHORT : INF_ERR
 	for (;;) {
 		if (header) { // byte-aligned here
 			const uint64_t at = in.pos() >> 3;
 			const int64_t d = inf_gzip_header(gz, n, at);
-			if (d < 0) return INF_ERR;
+			if (d < 0) return d == -2 ? INF_SHORT : INF_ERR;
 			in.init(gz, n, (uint64_t)d * 8);
 			o.member_start();
 			header = false;
@@ -378,43 +381,44 @@ INF_HD_NOINL int inf_run(const uint8_t *gz, uint64_t n, uint64_t bit, bool at_he
 		if (btype == 0) {
 			in.align();
 			const uint32_t len = in.bits(16), nlen = in.bits(16);
-			if ((len ^ 0xffffu) != nlen || in.over()) return INF_ERR;
+			if (in.over()) return INF_SHORT;
+			if ((len ^ 0xffffu) != nlen) return INF_ERR;
 			const uint64_t at = in.pos() >> 3;
-			if (at > n || len > n - at) return INF_ERR;
+			if (at > n || len > n - at) return INF_SHORT;
 			for (uint32_t k = 0; k < len; ++k) if (!o.lit(gz[at + k])) return INF_ERR;
 			in.init(gz, n, (at + len) * 8);
 		} else if (btype == 3) {
-			return INF_ERR;
+			INF_FAIL;
 		} else {
 			if (btype == 1) { if (t.kind != 1) inf_build_fixed(t, true); }
-			else if (!inf_read_dynamic(in, t, false, true)) return INF_ERR;
+			else if (!inf_read_dynamic(in, t, false, true)) INF_FAIL;
 			for (;;) {
 				in.refill();
 				const int s = t.lit.decode(in, true);
 				if (s < 256) {
-					if (s < 0 || !o.lit((uint32_t)s)) return INF_ERR;
+					if (s < 0 || !o.lit((uint32_t)s)) INF_FAIL;
 				} else if (s == 256) {
 					break;
 				} else {
-					if (s > 285) return INF_ERR;
+					if (s > 285) INF_FAIL;
 					int base, extra, dbase, dextra;
 					inf_len_code(s - 257, base, extra);
 					const int len = base + (int)in.bits(extra);
 					const int ds = t.dist.decode(in, true);
-					if (ds < 0 || ds > 29) return INF_ERR;
+					if (ds < 0 || ds > 29) INF_FAIL;
 					inf_dist_code(ds, dbase, dextra);
 					const int dist = dbase + (int)in.bits(dextra);
-					if (in.over() || !o.copy(len, dist)) return INF_ERR;
+					if (in.over() || !o.copy(len, dist)) INF_FAIL;
 				}
-				if (in.over()) return INF_ERR;
+				if (in.over()) return INF_SHORT;
 			}
 			if (btype == 2) t.kind = 0;
 		}
-		if (in.over()) return INF_ERR;
+		if (in.over()) return INF_SHORT;
 		if (bfinal) { // trailer: CRC-32, ISIZE; then the end of the input or the next member
 			in.align();
 			const uint64_t at = in.pos() >> 3;
-			if (at > n || n - at < 8) return INF_ERR;
+			if (at > n || n - at < 8) return INF_SHORT;
 			const uint8_t *q = gz + at;
 			const uint32_t crc = q[0] | q[1] << 8 | q[2] << 16 | (uint32_t)q[3] << 24;
 			const uint32_t isz = q[4] | q[5] << 8 | q[6] << 16 | (uint32_t)q[7] << 24;
@@ -424,6 +428,7 @@ INF_HD_NOINL int inf_run(const uint8_t *gz, uint64_t n, uint64_t bit, bool at_he
 			header = true;
 		}
 	}
+#undef INF_FAIL
 }
 
 // ---- window step: byte k of the 32 KiB window that follows a unit, from its pass-1 ring and the window that precedes it -----

@@ -1630,7 +1630,18 @@ __global__ void k_win_rank(const unsigned long long *first_sorted, const uint64_
 	if (threadIdx.x == 0 && s) atomicAdd(tot_len, s);
 }
 
-// The two windows on both sides of PCIe and what a launch over one of them needs.
+// one past the last '\n' of p[0, n) (device memory), 0 if there is none
+__global__ void k_last_nl(const char *p, uint64_t n, unsigned long long *out)
+{
+	unsigned long long best = 0;
+	for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) if (p[i] == '\n') best = i + 1;
+	typedef cub::BlockReduce<unsigned long long, 256> BR;
+	__shared__ typename BR::TempStorage t;
+	best = BR(t).Reduce(best, cub::Max());
+	if (threadIdx.x == 0 && best) atomicMax(out, best);
+}
+
+// The two windows on both sides of PCIe and what a launch over one of them needs (a device source: the device windows only).
 struct WinRun {
 	MabDev &d;
 	const TextSource &src;
@@ -1640,7 +1651,7 @@ struct WinRun {
 	void *ts_mem = nullptr;
 	LineTileState ts;
 	unsigned *ctr = nullptr;
-	unsigned long long *ws = nullptr;
+	unsigned long long *ws = nullptr, *nl = nullptr;
 
 	WinRun(MabDev &dev_, const TextSource &s, size_t w) : d(dev_), src(s), cap(0)
 	{
@@ -1650,6 +1661,7 @@ struct WinRun {
 		}
 		ctr = mab_alloc<unsigned>(d, 1);
 		ws = (unsigned long long*)mab_alloc<uint64_t>(d, WS_N);
+		nl = (unsigned long long*)mab_alloc<uint64_t>(d, 1);
 		if (!d.copy_stream) MAB_CUDA(cudaStreamCreateWithFlags(&d.copy_stream, cudaStreamNonBlocking));
 		resize(w, 0, 0);
 	}
@@ -1658,24 +1670,29 @@ struct WinRun {
 		d.sync();
 		MAB_CUDA(cudaStreamSynchronize(d.copy_stream));
 		for (int i = 0; i < 2; ++i) {
-			MAB_CUDA(cudaFreeHost(host[i]));
+			if (host[i]) MAB_CUDA(cudaFreeHost(host[i]));
 			d.free(dev[i]);
 			MAB_CUDA(cudaEventDestroy(copied[i])); MAB_CUDA(cudaEventDestroy(parsed[i]));
 		}
-		d.free(ts_mem); d.free(ctr); d.free(ws);
+		d.free(ts_mem); d.free(ctr); d.free(ws); d.free(nl);
 	}
-	// windows of w bytes, keeping the first `keep` bytes of host window b (nothing is in flight when it is called with cap != 0)
+	// windows of w bytes, keeping the first `keep` bytes of window b (host, or device for a device source; nothing is in flight
+	// when it is called with cap != 0)
 	void resize(size_t w, int b, size_t keep)
 	{
 		if (cap) { d.sync(); MAB_CUDA(cudaStreamSynchronize(d.copy_stream)); }
 		for (int i = 0; i < 2; ++i) {
-			char *nh;
-			MAB_CUDA(cudaMallocHost(&nh, w));
-			if (i == b && keep) memcpy(nh, host[i], keep);
-			if (host[i]) MAB_CUDA(cudaFreeHost(host[i]));
-			host[i] = nh;
-			if (dev[i]) d.free(dev[i]);
+			if (!src.fill) {
+				char *nh;
+				MAB_CUDA(cudaMallocHost(&nh, w));
+				if (i == b && keep) memcpy(nh, host[i], keep);
+				if (host[i]) MAB_CUDA(cudaFreeHost(host[i]));
+				host[i] = nh;
+			}
+			char *old = dev[i];
+			if (!(src.fill && i == b && keep) && old) d.free(old), old = nullptr;
 			dev[i] = (char*)d.alloc(w + 64);                      // (+64: the tiles are staged in whole 16-byte words)
+			if (old) { MAB_CUDA(cudaMemcpyAsync(dev[i], old, keep, cudaMemcpyDeviceToDevice, d.stream)); d.free(old); }
 		}
 		if (ts_mem) d.free(ts_mem);
 		ts = tiles_alloc(d, w / PT_TILE + 1, &ts_mem);
@@ -1698,6 +1715,53 @@ static bool win_pass(WinRun &w, int min_span, int min_match, int bi_dir, const W
 	const char *tail = nullptr;                                 // the unfinished line after the previous window, still in its host buffer
 	size_t n_tail = 0, total = 0;
 	bool eof = false;
+	if (w.src.fill) { // a device source: the windows are filled on the device, the unfinished line moves device to device
+		size_t tail_at = 0;
+		for (int b = 0; !eof; b ^= 1) {
+			if (n_tail) MAB_CUDA(cudaMemcpyAsync(w.dev[b], w.dev[b ^ 1] + tail_at, n_tail, cudaMemcpyDeviceToDevice, d.stream)); // (after window b's last launch: one stream)
+			size_t have = n_tail, cut = 0;
+			for (;;) {
+				while (have < w.cap) {
+					const int64_t r = w.src.fill(w.src.ud, w.dev[b] + have, w.cap - have);
+					if (r == TS_FULL) break;
+					if (r < 0) {
+						if (PASS == 2) { fprintf(stderr, "[E::miniasm_b200] the PAF source failed when read again after %llu bytes\n", (unsigned long long)total); exit(78); }
+						d.sync();
+						MAB_CUDA(cudaEventDestroy(ready));
+						return false;
+					}
+					if (r == 0) { eof = true; break; }
+					have += (size_t)r, total += (size_t)r;
+				}
+				if (eof) { cut = have; break; }
+				if (have) {
+					MAB_CUDA(cudaMemsetAsync(w.nl, 0, 8, d.stream));
+					const size_t look = have < (1u << 20) ? have : (1u << 20); // the last MB first, all of it if that has no line end
+					MAB_LAUNCH(d, k_last_nl, mab_grid(look, 256), 256, 0, w.dev[b] + (have - look), (uint64_t)look, w.nl);
+					unsigned long long nl = 0;
+					MAB_CUDA(cudaMemcpyAsync(&nl, w.nl, 8, cudaMemcpyDeviceToHost, d.stream));
+					d.sync();
+					if (nl) nl += have - look;
+					else if (look < have) {
+						MAB_LAUNCH(d, k_last_nl, mab_grid(have - look, 256), 256, 0, w.dev[b], (uint64_t)(have - look), w.nl);
+						MAB_CUDA(cudaMemcpyAsync(&nl, w.nl, 8, cudaMemcpyDeviceToHost, d.stream));
+						d.sync();
+					}
+					if (nl) { cut = (size_t)nl; break; }
+				}
+				w.resize(2 * w.cap, b, have);                       // a line longer than the window: the windows grow
+				if (tab.store_cap + w.cap >= (1ull << NT_OFF_BITS) - 1) { fprintf(stderr, "[E::miniasm_b200] more than 2^37 bytes of read names and window\n"); exit(73); }
+			}
+			tail_at = cut, n_tail = have - cut;
+			if (cut == 0) break;
+			const uint64_t n_tile = (cut + PT_TILE - 1) / PT_TILE;
+			tiles_reset(d, w.ts, n_tile);
+			MAB_CUDA(cudaMemsetAsync(w.ctr, 0, 4, d.stream));
+			MAB_LAUNCH(d, k_win_tiles<PASS>, (unsigned)n_tile, PT_THREADS, 0, w.dev[b], cut, w.ctr, w.ts, min_span, min_match, bi_dir, tab, bfirst, cur, out, w.ws);
+			MAB_CUDA(cudaMemcpyAsync(w.ws + WS_LINE_IN, w.ws + WS_LINE_OUT, 16, cudaMemcpyDeviceToDevice, d.stream));
+			MAB_CUDA(cudaEventRecord(w.parsed[b], d.stream));
+		}
+	}
 	for (int b = 0; !eof; b ^= 1) {
 		MAB_CUDA(cudaEventSynchronize(w.copied[b]));            // the window that last used this host buffer has crossed
 		if (n_tail) memcpy(w.host[b], tail, n_tail);

@@ -34,7 +34,14 @@ void ingest_paf_stream(MabDev &d, char *d_text, const char *host_text, size_t le
 // dictionary, a packed name store and the hits, never the text.  Same hits, names (names.off indexes *name_text_out, which the
 // caller frees) and counters as ingest_paf.  size_hint: bytes of the text when known (sizes the dictionary), else 0.
 // false: the source could not be rewound and nothing was ingested.  A source whose second delivery differs exits with code 78.
-struct TextSource { size_t (*read)(void *ud, char *dst, size_t cap); int (*rewind)(void *ud); void *ud; };
+// A device source (read == nullptr, fill set) writes the text straight into the device windows on the ingest's stream: fill returns
+// the bytes written (0 at the end), TS_FULL when its next piece is longer than cap (the window is cut at its last line, or grows),
+// or TS_FAIL; a TS_FAIL in pass 1 gives false with nothing ingested, in pass 2 exit 78.
+enum { TS_FULL = -3, TS_FAIL = -2 };
+struct TextSource {
+	size_t (*read)(void *ud, char *dst, size_t cap); int (*rewind)(void *ud); void *ud;
+	int64_t (*fill)(void *ud, char *d_dst, size_t cap);
+};
 bool ingest_paf_windowed(MabDev &d, const TextSource &src, size_t window_bytes, size_t size_hint, int min_span, int min_match, int bi_dir,
                          DHits &h, DNames &names, char **name_text_out, IngestStats &st);
 void names_free(MabDev &d, DNames &n);
