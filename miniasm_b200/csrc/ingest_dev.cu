@@ -250,10 +250,11 @@ __device__ __forceinline__ uint32_t tab_insert(const NameTab &t, const char *__r
 //   * stages its tile and PT_OVER bytes after it in shared memory with 128-bit loads (byte-wise walking of global
 //     memory makes every warp-level load touch ~16 cache lines),
 //   * counts the line starts of the tile there and publishes the count; a single-pass decoupled look-back over the
-//     tiles (cub::TilePrefixCallbackOp) returns the global number of its first line,
-//   * lists the starts and hands one line to each thread, which parses it, applies the store filter of hit.c:85 and
-//     enters both names into the dictionary while the line is still in shared memory, then writes start[line] and the
-//     32-byte record, and (optionally) adds the line's hits to the bucket sizes of its slots.
+//     tiles (cub::TilePrefixCallbackOp) returns the number of its first line,
+//   * lists the starts and hands one line to each thread, which parses it and applies the store filter of hit.c:85 while
+//     the line is still in shared memory, then hands it to the policy P (what the line leaves behind: ParseStore below, and
+//     the two passes of the windowed ingest, WinParse), and (when P has a count array) adds the line's hits to the bucket
+//     sizes of its slots.
 // The tile's last line is the only one that can end past the staged bytes: it is parsed straight from global memory.
 // Lines numbered line_cap or more are counted but not parsed (the host parses again with room for all of them).
 constexpr int PT_THREADS = 128;
@@ -282,10 +283,18 @@ __device__ __forceinline__ uint32_t nl_bits_u4(const uint4 w)  // bit k = byte k
 __global__ void k_tiles_init(LineTileState ts, int n_tile) { ts.InitializeStatus(n_tile); }
 
 // Tiles [t_lo, t_lo + gridDim.x) of the text, one per CTA.  avail: bytes of the text present (== len unless the text is still
-// arriving, and then at least PT_TILE past the last tile of the launch).
+// arriving, and then at least PT_TILE past the last tile of the launch).  P is what a line leaves behind; it provides
+//   line_base()        the number of the text's first line;
+//   lines_end(n)       called by the text's last tile: the text ends before line n;
+//   cut()              the tile's last line runs past the bytes that have arrived (it is not parsed);
+//   hits()             the per-slot hit counts to add the line's hits to, or nullptr;
+//   line(...)          the action on line i, parsed from base + [s, eol) (base + offset = address of that byte of the text);
+//                      stored: it passed the store filter; sq, st: the slots its hits are counted on (NOSLOT: none);
+//   flush(lane, ...)   called by every lane at the end of the CTA with the warp's totals of parsed and stored lines.
+template <class P>
 __global__ void __launch_bounds__(PT_THREADS)
-k_parse_tiles(const char *__restrict__ text, size_t len, size_t avail, uint64_t t_lo, unsigned *tile_ctr, LineTileState tstate,
-              int min_span, int min_match, int bi_dir, NameTab tab, PRec *out, uint64_t *start, uint64_t line_cap, unsigned long long *counts)
+k_parse_tiles(const char *__restrict__ text, size_t len, size_t avail, uint64_t t_lo, uint64_t line_cap, unsigned *tile_ctr, LineTileState tstate,
+              int min_span, int min_match, int bi_dir, P pol)
 {
 	typedef cub::BlockScan<uint32_t, PT_THREADS> BS;
 	__shared__ __align__(16) char s_text[PT_TILE + PT_OVER + 16];  // (+16: parse_line reads whole aligned words)
@@ -328,8 +337,8 @@ k_parse_tiles(const char *__restrict__ text, size_t len, size_t avail, uint64_t 
 		}
 	}
 	__syncthreads();
-	const uint64_t first = s_first;
-	if (threadIdx.x == 0 && b1 == len) counts[PC_LINES] = first + n;
+	const uint64_t first = pol.line_base() + s_first;
+	if (threadIdx.x == 0 && b1 == len) pol.lines_end(first + n);
 	if (n == 0) return;
 	uint64_t last_eol = s_nl != ~0u ? b0 + s_nl : w_end >= len ? len : ~0ull; // ~0: not staged, ends past the overhang
 	if (last_eol == ~0ull) { // (the same for the whole CTA) warp 0 looks for the end of that long line in global memory
@@ -345,7 +354,7 @@ k_parse_tiles(const char *__restrict__ text, size_t len, size_t avail, uint64_t 
 			if (e == ~0ull && avail == len) e = len;
 			if (threadIdx.x == 0) {
 				s_eol = e;
-				if (e == ~0ull) atomicAdd(counts + PC_CUT, 1ull); // it runs past the bytes that have arrived
+				if (e == ~0ull) pol.cut();
 			}
 		}
 		__syncthreads();
@@ -370,37 +379,60 @@ k_parse_tiles(const char *__restrict__ text, size_t len, size_t avail, uint64_t 
 				const uint64_t s = b0 + s_start[j];
 				uint64_t eol = r0 + j + 1 < n ? b0 + s_start[j + 1] - 1 : last_eol;
 				if (eol != ~0ull) {
-					const char *base = eol <= w_end ? s_text - b0 : text; // base + file offset = address of that byte
+					const char *base = eol <= w_end ? s_text - b0 : text;
 					if (eol - s > 1 && base[eol - 1] == '\r') --eol;
 					PLine r;
 					parse_line(base + s, base + eol, r, &s_vals[threadIdx.x >> 5][0][lane]);
+					bool stored = false;
 					if (r.nf >= 10) {
 						++n_parsed;
-						if (!(r.qe - r.qs < (uint32_t)min_span || r.te - r.ts < (uint32_t)min_span || (int)(r.ml_rev & 0x7fffffffu) < min_match)) {
-							++n_pass;
-							sq = tab_insert(tab, text, base + s, r.qnl, s, 2 * i, counts + PC_OVERFLOW);
-							st = tab_insert(tab, text, base + s + r.tdelta, r.tnl, s + r.tdelta, 2 * i + 1, counts + PC_OVERFLOW);
-						}
+						stored = !(r.qe - r.qs < (uint32_t)min_span || r.te - r.ts < (uint32_t)min_span || (int)(r.ml_rev & 0x7fffffffu) < min_match);
+						n_pass += stored;
 					}
-					start[i] = s;
-					*reinterpret_cast<uint4*>(out + i) = make_uint4(r.qs, r.qe, r.ts, r.te);
-					*(reinterpret_cast<uint4*>(out + i) + 1) = make_uint4(r.ml_rev, (r.bl & 0x7fffffffu) | (r.nf >= 11 ? 0x80000000u : 0u), sq, st);
+					pol.line(text, base, s, i, r, stored, bi_dir, sq, st);
 				}
 			}
-			if (tab.hits) { // consecutive lines often share their query read: one add per distinct slot of the warp
+			if (uint32_t *hits = pol.hits()) { // consecutive lines often share their query read: one add per distinct slot of the warp
 				const unsigned grp = __match_any_sync(0xffffffffu, sq);
-				if (sq != NOSLOT && lane == (uint32_t)__ffs(grp) - 1) atomicAdd(&tab.hits[sq], (uint32_t)__popc(grp));
-				if (sq != NOSLOT && bi_dir && st != sq) atomicAdd(&tab.hits[st], 1u);
+				if (sq != NOSLOT && lane == (uint32_t)__ffs(grp) - 1) atomicAdd(&hits[sq], (uint32_t)__popc(grp));
+				if (sq != NOSLOT && bi_dir && st != sq) atomicAdd(&hits[st], 1u);
 			}
 		}
 		__syncthreads(); // the list is rewritten by the next round
 	}
-	n_parsed = __reduce_add_sync(0xffffffffu, n_parsed), n_pass = __reduce_add_sync(0xffffffffu, n_pass);
-	if (lane == 0) {
-		if (n_parsed) atomicAdd(counts + PC_PARSED, (unsigned long long)n_parsed);
-		if (n_pass) atomicAdd(counts + PC_STORED, (unsigned long long)n_pass);
-	}
+	pol.flush(lane, __reduce_add_sync(0xffffffffu, n_parsed), __reduce_add_sync(0xffffffffu, n_pass));
 }
+
+// The resident and the streamed parse: start[line] and the 32-byte record of every line, both names of a stored line into the
+// dictionary; counts[] as PC_*.
+struct ParseStore {
+	NameTab tab;
+	PRec *out;
+	uint64_t *start;
+	unsigned long long *counts;
+
+	__device__ __forceinline__ uint64_t line_base() const { return 0; }
+	__device__ __forceinline__ void lines_end(uint64_t n) const { counts[PC_LINES] = n; }
+	__device__ __forceinline__ void cut() const { atomicAdd(counts + PC_CUT, 1ull); }
+	__device__ __forceinline__ uint32_t *hits() const { return tab.hits; }
+	__device__ __forceinline__ void line(const char *text, const char *base, uint64_t s, uint64_t i, const PLine &r, bool stored, int, uint32_t &sq, uint32_t &st)
+	{
+		if (stored) {
+			sq = tab_insert(tab, text, base + s, r.qnl, s, 2 * i, counts + PC_OVERFLOW);
+			st = tab_insert(tab, text, base + s + r.tdelta, r.tnl, s + r.tdelta, 2 * i + 1, counts + PC_OVERFLOW);
+		}
+		start[i] = s;
+		*reinterpret_cast<uint4*>(out + i) = make_uint4(r.qs, r.qe, r.ts, r.te);
+		*(reinterpret_cast<uint4*>(out + i) + 1) = make_uint4(r.ml_rev, (r.bl & 0x7fffffffu) | (r.nf >= 11 ? 0x80000000u : 0u), sq, st);
+	}
+	__device__ __forceinline__ void flush(uint32_t lane, unsigned n_parsed, unsigned n_pass) const
+	{
+		if (lane == 0) {
+			if (n_parsed) atomicAdd(counts + PC_PARSED, (unsigned long long)n_parsed);
+			if (n_pass) atomicAdd(counts + PC_STORED, (unsigned long long)n_pass);
+		}
+	}
+};
 
 // bl of a 10-field line: the value of the closest earlier line that had an 11th field (paf.c:47, hit.c:73);
 // carry_bl = what the lines before this rank's byte range left behind (sharded runs), else 0
@@ -477,9 +509,9 @@ __global__ void k_count_u8(const uint8_t *a, uint64_t n, unsigned long long *out
 	if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, (unsigned long long)c);
 }
 
-__global__ void k_dict_pairs(const uint64_t *slots, uint32_t n, NameTab t, unsigned long long *first_out)
+__global__ void k_slot_first(const uint64_t *slots, uint32_t n, const unsigned long long *first, unsigned long long *first_out)
 {
-	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) first_out[i] = t.first[slots[i]];
+	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) first_out[i] = first[slots[i]];
 }
 
 // read_cnt[id] = hits of the read (slot -> id is a permutation: the per-slot counts of the parse become per-read counts here)
@@ -550,7 +582,90 @@ void names_free(MabDev &d, DNames &n)
 	n = DNames();
 }
 
+// room for the names of n reads; read ids are 31-bit
+static uint32_t names_alloc(MabDev &d, DNames &names, uint64_t n)
+{
+	if (n >= (1ull << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 reads\n"); exit(73); }
+	names.n_seq = (uint32_t)n;
+	names.off = mab_alloc<uint64_t>(d, n); names.nlen = mab_alloc<uint32_t>(d, n); names.slen = mab_alloc<uint32_t>(d, n);
+	return (uint32_t)n;
+}
+
+// Every ingest starts from nothing.  text_len: bytes of text held at once, whose offsets a dictionary word keeps in NT_OFF_BITS
+// (0 for the windowed ingest, which checks its name store and window instead).
+static void ingest_open(size_t text_len, DHits &h, DNames &names, IngestStats &st)
+{
+	memset(&st, 0, sizeof(st));
+	names = DNames();
+	h.n = 0, h.n_seq = 0;
+	if (text_len >= (1ull << NT_OFF_BITS) - 1) { fprintf(stderr, "[E::miniasm_b200] more than 2^37 bytes of PAF on one GPU\n"); exit(73); }
+}
+
 static inline uint32_t bits_for(uint64_t x) { uint32_t b = 0; while (x) ++b, x >>= 1; return b ? b : 1; }
+
+// The slots in [0, cap) that `used` keeps, in slot order; returns how many.
+template <class Used>
+static uint64_t list_slots(MabDev &d, uint64_t cap, Used used, uint64_t *slots)
+{
+	cub::CountingInputIterator<uint64_t> pos(0);
+	size_t tb = 0;
+	unsigned long long *d_n = d.d_scal + SC_NSEL;
+	cub::DeviceSelect::If(nullptr, tb, pos, slots, d_n, (int64_t)cap, used, d.stream);
+	void *tmp = d.tmp(tb);
+	cub::DeviceSelect::If(tmp, tb, pos, slots, d_n, (int64_t)cap, used, d.stream);
+	++d.n_lib;
+	return d.get_scal(SC_NSEL);
+}
+
+// ids = rank of the first occurrence: the n listed slots are sorted by bits [lo_bit, hi_bit) of first[slot] (the occurrence
+// number) and rank(first_sorted, slot_sorted, n, tot_len) gives every slot its position as id and adds the reads' lengths to
+// *tot_len.  Returns that sum.  `slots` is sort scratch afterwards.
+template <class Rank>
+static unsigned long long rank_slots(MabDev &d, uint64_t *slots, uint32_t n, const unsigned long long *first, int lo_bit, int hi_bit, Rank rank)
+{
+	if (!n) return 0;
+	unsigned long long *fa = (unsigned long long*)mab_alloc<uint64_t>(d, n), *fb = (unsigned long long*)mab_alloc<uint64_t>(d, n);
+	uint64_t *sb = mab_alloc<uint64_t>(d, n);
+	MAB_LAUNCH(d, k_slot_first, mab_grid(n, 256), 256, 0, slots, n, first, fa);
+	cub::DoubleBuffer<unsigned long long> dk(fa, fb);
+	cub::DoubleBuffer<uint64_t> dv(slots, sb);
+	size_t tb = 0;
+	cub::DeviceRadixSort::SortPairs(nullptr, tb, dk, dv, (int)n, lo_bit, hi_bit, d.stream);
+	void *tmp = d.tmp(tb);
+	cub::DeviceRadixSort::SortPairs(tmp, tb, dk, dv, (int)n, lo_bit, hi_bit, d.stream);
+	++d.n_lib;
+	d.zero_scal(SC_AUX, 1);
+	rank(dk.Current(), dv.Current(), n, d.d_scal + SC_AUX);
+	const unsigned long long tot_len = d.get_scal(SC_AUX);
+	d.free(fa); d.free(fb); d.free(sb);
+	return tot_len;
+}
+
+// The reads of a single-GPU ingest: the used slots of `tab` (cap slots) are ranked as in rank_slots, rank(..., read_cnt) also
+// writing every read's hit count.  The counts become the bucket starts of the hit array (*bfirst, n_seq + 1 words) and then,
+// zeroed, the buckets' fill cursors (*cur); h gets room for all the hits.
+template <class Rank>
+static void rank_reads(MabDev &d, const NameTab &tab, uint64_t cap, int lo_bit, int hi_bit, Rank rank, DHits &h, DNames &names, IngestStats &st,
+                       uint32_t *&cur, uint32_t *&bfirst)
+{
+	uint64_t *slots = mab_alloc<uint64_t>(d, cap);
+	const uint32_t n_seq = names_alloc(d, names, list_slots(d, cap, SlotUsed{tab.first}, slots));
+	uint32_t *read_cnt = mab_alloc<uint32_t>(d, (size_t)n_seq + 1), *first = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);
+	MAB_CUDA(cudaMemsetAsync(read_cnt + n_seq, 0, 4, d.stream));
+	st.tot_len = rank_slots(d, slots, n_seq, tab.first, lo_bit, hi_bit,
+	                        [&](const unsigned long long *fs, const uint64_t *ss, uint32_t n, unsigned long long *tot) { rank(fs, ss, n, tot, read_cnt); });
+	d.free(slots);
+	d.trace("ingest:rank_ids");
+	dh_bucket_first(d, read_cnt, n_seq, first);
+	MAB_CUDA(cudaMemsetAsync(read_cnt, 0, (size_t)n_seq * 4, d.stream)); // the counts become the buckets' fill cursors
+	uint32_t n_hits;
+	MAB_CUDA(cudaMemcpyAsync(&n_hits, first + n_seq, 4, cudaMemcpyDeviceToHost, d.stream));
+	d.sync();
+	dh_reserve(d, h, n_hits ? n_hits : 1);
+	h.n = n_hits, h.n_seq = n_seq;
+	st.n_hits = n_hits, st.n_seq = n_seq;
+	cur = read_cnt, bfirst = first;
+}
 
 static NameTab tab_alloc(MabDev &d, uint64_t cap, bool with_hits)
 {
@@ -623,8 +738,8 @@ static void parse_resident(MabDev &d, const char *d_text, size_t len, int min_sp
 		if (n_tile) {
 			tiles_reset(d, ts, n_tile);
 			MAB_CUDA(cudaMemsetAsync(ctr, 0, 4, d.stream));
-			MAB_LAUNCH(d, k_parse_tiles, (unsigned)n_tile, PT_THREADS, 0, d_text, len, len, 0, ctr, ts, min_span, min_match, bi_dir, p.tab, p.ln, p.start,
-			           line_cap, d.d_scal + SC_COUNT);
+			MAB_LAUNCH(d, k_parse_tiles<ParseStore>, (unsigned)n_tile, PT_THREADS, 0, d_text, len, len, 0, line_cap, ctr, ts, min_span, min_match, bi_dir,
+			           ParseStore{p.tab, p.ln, p.start, d.d_scal + SC_COUNT});
 		}
 		p.n_parsed = d.get_scal(SC_COUNT + PC_PARSED);
 		p.n_lines = d.h_scal[SC_COUNT + PC_LINES];
@@ -645,11 +760,8 @@ static void ingest_finish(MabDev &d, const char *d_text, size_t len, uint64_t *s
 void ingest_paf(MabDev &d, const char *d_text, size_t len, int min_span, int min_match, int bi_dir, DHits &h, DNames &names, IngestStats &st,
                 const NoContParams *nocont)
 {
-	memset(&st, 0, sizeof(st));
-	names = DNames();
-	h.n = 0, h.n_seq = 0;
+	ingest_open(len, h, names, st);
 	if (len == 0) { dh_reserve(d, h, 1); return; }
-	if (len >= (1ull << NT_OFF_BITS) - 1) { fprintf(stderr, "[E::miniasm_b200] more than 2^37 bytes of PAF on one GPU\n"); exit(73); }
 
 	d.trace("ingest:begin");
 	// (1)+(2) line starts, parse, store filter, dictionary insert and hit counts per name in one pass
@@ -696,8 +808,8 @@ static bool stream_parse(MabDev &d, char *d_text, const char *host_text, size_t 
 		MAB_CUDA(cudaEventRecord(ev[k], d.copy_stream));
 		MAB_CUDA(cudaStreamWaitEvent(d.stream, ev[k], 0));
 		const uint64_t t_hi = k + 1 == n_chunk ? n_tile : t1 - 1;
-		MAB_LAUNCH(d, k_parse_tiles, (unsigned)(t_hi - t_done), PT_THREADS, 0, d_text, len, b1, t_done, ctr + k, ts, min_span, min_match, bi_dir, p.tab, p.ln,
-		           p.start, line_cap, d.d_scal + SC_COUNT);
+		MAB_LAUNCH(d, k_parse_tiles<ParseStore>, (unsigned)(t_hi - t_done), PT_THREADS, 0, d_text, len, b1, t_done, line_cap, ctr + k, ts, min_span, min_match,
+		           bi_dir, ParseStore{p.tab, p.ln, p.start, d.d_scal + SC_COUNT});
 		t_done = t_hi;
 	}
 	p.n_parsed = d.get_scal(SC_COUNT + PC_PARSED);               // (synchronises)
@@ -719,11 +831,8 @@ static bool stream_parse(MabDev &d, char *d_text, const char *host_text, size_t 
 void ingest_paf_stream(MabDev &d, char *d_text, const char *host_text, size_t len, int min_span, int min_match, int bi_dir,
                        DHits &h, DNames &names, IngestStats &st)
 {
-	memset(&st, 0, sizeof(st));
-	names = DNames();
-	h.n = 0, h.n_seq = 0;
+	ingest_open(len, h, names, st);
 	if (len == 0) { dh_reserve(d, h, 1); return; }
-	if (len >= (1ull << NT_OFF_BITS) - 1) { fprintf(stderr, "[E::miniasm_b200] more than 2^37 bytes of PAF on one GPU\n"); exit(73); }
 	Parsed p;
 	if (!stream_parse(d, d_text, host_text, len, min_span, min_match, bi_dir, true, p)) {
 		ingest_paf(d, d_text, len, min_span, min_match, bi_dir, h, names, st, nullptr); // the text is resident now: the plain path parses it again
@@ -755,56 +864,12 @@ static void ingest_finish(MabDev &d, const char *d_text, size_t len, uint64_t *s
 		d.trace("ingest:-R prefilter");
 	}
 	// (4) ids = rank of the first occurrence; the hit counts of the slots become those of the reads (the bucket sizes of the sort)
-	uint64_t *slots = mab_alloc<uint64_t>(d, cap);
-	uint32_t n_seq;
-	{
-		cub::CountingInputIterator<uint64_t> pos(0);
-		SlotUsed used{tab.first};
-		size_t tb = 0;
-		unsigned long long *d_n = d.d_scal + SC_NSEL;
-		cub::DeviceSelect::If(nullptr, tb, pos, slots, d_n, (int64_t)cap, used, d.stream);
-		void *tmp = d.tmp(tb);
-		cub::DeviceSelect::If(tmp, tb, pos, slots, d_n, (int64_t)cap, used, d.stream);
-		++d.n_lib;
-		uint64_t n = d.get_scal(SC_NSEL);
-		if (n >= (1ull << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 reads\n"); exit(73); }
-		n_seq = (uint32_t)n;
-	}
-	names.n_seq = n_seq;
-	names.off = mab_alloc<uint64_t>(d, n_seq); names.nlen = mab_alloc<uint32_t>(d, n_seq); names.slen = mab_alloc<uint32_t>(d, n_seq);
-	uint32_t *read_cnt = mab_alloc<uint32_t>(d, (size_t)n_seq + 1), *first = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);
-	MAB_CUDA(cudaMemsetAsync(read_cnt + n_seq, 0, 4, d.stream));
-	if (n_seq) {
-		unsigned long long *fa = (unsigned long long*)mab_alloc<uint64_t>(d, n_seq), *fb = (unsigned long long*)mab_alloc<uint64_t>(d, n_seq);
-		uint64_t *sb = mab_alloc<uint64_t>(d, n_seq);
-		MAB_LAUNCH(d, k_dict_pairs, mab_grid(n_seq, 256), 256, 0, slots, n_seq, tab, fa);
-		cub::DoubleBuffer<unsigned long long> dk(fa, fb);
-		cub::DoubleBuffer<uint64_t> dv(slots, sb);
-		size_t tb = 0;
-		int end_bit = (int)bits_for(2 * n_lines + 1);
-		cub::DeviceRadixSort::SortPairs(nullptr, tb, dk, dv, (int)n_seq, 0, end_bit, d.stream);
-		void *tmp = d.tmp(tb);
-		cub::DeviceRadixSort::SortPairs(tmp, tb, dk, dv, (int)n_seq, 0, end_bit, d.stream);
-		++d.n_lib;
-		d.zero_scal(SC_AUX, 1);
-		MAB_LAUNCH(d, k_dict_rank, mab_grid(n_seq, 256), 256, 0, dk.Current(), dv.Current(), n_seq, tab, d_text, start, names.off, names.nlen, names.slen, d.d_scal + SC_AUX,
-		           read_cnt);
-		st.tot_len = d.get_scal(SC_AUX);
-		d.free(fa); d.free(fb); d.free(sb);
-	}
-	d.free(slots);
-
-	d.trace("ingest:rank_ids");
+	uint32_t *read_cnt, *first;
+	rank_reads(d, tab, cap, 0, (int)bits_for(2 * n_lines + 1), [&](const unsigned long long *fs, const uint64_t *ss, uint32_t n, unsigned long long *tot, uint32_t *cnt) {
+		MAB_LAUNCH(d, k_dict_rank, mab_grid(n, 256), 256, 0, fs, ss, n, tab, d_text, start, names.off, names.nlen, names.slen, tot, cnt);
+	}, h, names, st, read_cnt, first);
 	// (5) every hit emitted straight into its read's bucket of h.a2
-	dh_bucket_first(d, read_cnt, n_seq, first);
-	MAB_CUDA(cudaMemsetAsync(read_cnt, 0, (size_t)n_seq * 4, d.stream)); // the counts become the buckets' fill cursors
-	uint32_t n_hits;
-	MAB_CUDA(cudaMemcpyAsync(&n_hits, first + n_seq, 4, cudaMemcpyDeviceToHost, d.stream));
-	d.sync();
-	dh_reserve(d, h, n_hits ? n_hits : 1);
-	h.n = n_hits, h.n_seq = n_seq;
-	if (n_hits) MAB_LAUNCH(d, k_hit_emit, mab_grid(n_lines, 256), 256, 0, ln, n_lines, bi_dir, tab, first, read_cnt, h.a2);
-	st.n_hits = n_hits, st.n_seq = n_seq;
+	if (h.n) MAB_LAUNCH(d, k_hit_emit, mab_grid(n_lines, 256), 256, 0, ln, n_lines, bi_dir, tab, first, read_cnt, h.a2);
 	d.free(ln); d.free(start);
 	tab_free(d, tab);
 
@@ -914,11 +979,6 @@ __global__ void k_gtab_verify(const GEntry *ent, uint64_t n, GTab t, const uint3
 }
 
 struct GSlotUsed { const unsigned long long *key; __device__ __forceinline__ bool operator()(uint64_t s) const { return key[s] != 0; } };
-
-__global__ void k_gtab_first(const uint64_t *slots, uint32_t n, GTab t, unsigned long long *first_out)
-{
-	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) first_out[i] = t.first[slots[i]];
-}
 
 __global__ void k_gtab_rank(const uint64_t *slot_sorted, uint32_t n, GTab t, const GEntry *ent, const uint64_t *name_pos,
                             uint64_t *noff, uint32_t *nlen, uint32_t *slen, unsigned long long *tot_len)
@@ -1089,12 +1149,9 @@ __global__ void k_iota32(uint32_t *a, uint64_t n) { for (uint64_t i = blockIdx.x
 void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int min_span, int min_match, int bi_dir,
                         DHits &h, DNames &names, char **name_text_out, IngestStats &st, const char *host_text)
 {	// host_text != nullptr: this rank's bytes are still on the host; they are copied in chunks while the arrived chunks are parsed
-	memset(&st, 0, sizeof(st));
-	names = DNames();
-	h.n = 0, h.n_seq = 0;
+	ingest_open(len, h, names, st);
 	const int G = sc.world;
 	// (1)+(2) local line starts, parse + store filter + local dictionary (exact: occurrences are compared with a witness in the text)
-	if (len >= (1ull << NT_OFF_BITS) - 1) { fprintf(stderr, "[E::miniasm_b200] more than 2^37 bytes of PAF on one GPU\n"); exit(73); }
 	Parsed p;
 	bool have = false;                                      // this rank holds a finished local parse
 	if (host_text && len) {
@@ -1125,19 +1182,8 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 	}
 	// (3) distinct names of this rank -> entries + packed names, all-gathered; (4) global table (replicated).  Two different names
 	// with one 64-bit hash would share a global slot: the byte comparison finds that and the entries are hashed again with another seed.
-	uint32_t n_ent = 0;
 	uint64_t *slots = mab_alloc<uint64_t>(d, cap);
-	{
-		cub::CountingInputIterator<uint64_t> pos(0);
-		SlotUsed used{tab.first};
-		size_t tb = 0;
-		unsigned long long *d_n = d.d_scal + SC_NSEL;
-		cub::DeviceSelect::If(nullptr, tb, pos, slots, d_n, (int64_t)cap, used, d.stream);
-		void *tmp = d.tmp(tb);
-		cub::DeviceSelect::If(tmp, tb, pos, slots, d_n, (int64_t)cap, used, d.stream);
-		++d.n_lib;
-		n_ent = (uint32_t)d.get_scal(SC_NSEL);
-	}
+	const uint32_t n_ent = (uint32_t)list_slots(d, cap, SlotUsed{tab.first}, slots);
 	GTab gt{nullptr, nullptr, nullptr, nullptr, 0};
 	GEntry *g_ent = nullptr;
 	char *g_names = nullptr;
@@ -1216,36 +1262,11 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 	{
 		const uint64_t gcap = gt.mask + 1;
 		uint64_t *slots = mab_alloc<uint64_t>(d, gcap);
-		cub::CountingInputIterator<uint64_t> pos(0);
-		GSlotUsed used{gt.key};
-		size_t tb = 0;
-		unsigned long long *d_n = d.d_scal + SC_NSEL;
-		cub::DeviceSelect::If(nullptr, tb, pos, slots, d_n, (int64_t)gcap, used, d.stream);
-		void *tmp = d.tmp(tb);
-		cub::DeviceSelect::If(tmp, tb, pos, slots, d_n, (int64_t)gcap, used, d.stream);
-		++d.n_lib;
-		uint64_t n = d.get_scal(SC_NSEL);
-		if (n >= (1ull << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 reads\n"); exit(73); }
-		n_seq = (uint32_t)n;
-		names.n_seq = n_seq;
-		names.off = mab_alloc<uint64_t>(d, n_seq); names.nlen = mab_alloc<uint32_t>(d, n_seq); names.slen = mab_alloc<uint32_t>(d, n_seq);
-		if (n_seq) {
-			unsigned long long *fa = (unsigned long long*)mab_alloc<uint64_t>(d, n_seq), *fb = (unsigned long long*)mab_alloc<uint64_t>(d, n_seq);
-			uint64_t *sb = mab_alloc<uint64_t>(d, n_seq);
-			MAB_LAUNCH(d, k_gtab_first, mab_grid(n_seq, 256), 256, 0, slots, n_seq, gt, fa);
-			cub::DoubleBuffer<unsigned long long> dk(fa, fb);
-			cub::DoubleBuffer<uint64_t> dv(slots, sb);
-			size_t tb2 = 0;
-			int end_bit = (int)bits_for(2 * n_lines_all + 1);
-			cub::DeviceRadixSort::SortPairs(nullptr, tb2, dk, dv, (int)n_seq, 0, end_bit, d.stream);
-			void *tmp2 = d.tmp(tb2);
-			cub::DeviceRadixSort::SortPairs(tmp2, tb2, dk, dv, (int)n_seq, 0, end_bit, d.stream);
-			++d.n_lib;
-			d.zero_scal(SC_AUX, 1);
-			MAB_LAUNCH(d, k_gtab_rank, mab_grid(n_seq, 256), 256, 0, dv.Current(), n_seq, gt, g_ent, g_pos, names.off, names.nlen, names.slen, d.d_scal + SC_AUX);
-			st.tot_len = d.get_scal(SC_AUX);
-			d.free(fa); d.free(fb); d.free(sb);
-		}
+		n_seq = names_alloc(d, names, list_slots(d, gcap, GSlotUsed{gt.key}, slots));
+		st.tot_len = rank_slots(d, slots, n_seq, gt.first, 0, (int)bits_for(2 * n_lines_all + 1),
+		                        [&](const unsigned long long *, const uint64_t *ss, uint32_t n, unsigned long long *tot) {
+			MAB_LAUNCH(d, k_gtab_rank, mab_grid(n, 256), 256, 0, ss, n, gt, g_ent, g_pos, names.off, names.nlen, names.slen, tot);
+		});
 		d.free(slots);
 	}
 	*name_text_out = g_names; // names.off points into this buffer (owned by the caller from now on)
@@ -1364,9 +1385,8 @@ void ingest_paf_sharded(MabDev &d, ShardComm &sc, char *d_text, size_t len, int 
 
 // =============================================================================================================
 // Windowed ingest: the text comes from a source that is read twice, one window at a time, so the device never holds more
-// of it than two windows (DESIGN.md 3d).  A window is a run of whole lines: it is numbered, parsed and filtered the way
-// k_parse_tiles does it (8 KB tiles staged in shared memory, decoupled look-back over the window's tiles), with the global
-// number of the window's first line carried from window to window in device memory.
+// of it than two windows (DESIGN.md 3d).  A window is a run of whole lines: k_parse_tiles<WinParse<PASS>> numbers, parses
+// and filters it, with the global number of the window's first line carried from window to window in device memory.
 //   pass 1  enters the names of the stored lines into the dictionary and counts the hits per name; no record is kept.  A
 //           name that is new is copied into the packed name store at once and its witness re-pointed there, so nothing
 //           refers to a window after its launch; first[slot] carries the sequence-length column of the occurrence it names.
@@ -1463,151 +1483,70 @@ __device__ uint32_t win_prev_bl(const char *text, uint64_t s, unsigned long long
 	return (uint32_t)carry & 0x7fffffffu;
 }
 
-// One window [text, text + len) of whole lines (the last window may lack the final '\n'), one tile per CTA.
-// PASS 2: bfirst = bucket starts per read id (n_seq + 1), cur = fill cursors, out = the hit buckets.
+// The windowed ingest's action on a line of a window [text, text + len) of whole lines (the last window may lack the final '\n'),
+// launched as k_parse_tiles<WinParse<PASS>> over all of the window: its lines are numbered on from ws[WS_LINE_IN].
+// PASS 1 enters the names of the stored lines and counts their hits; PASS 2 looks them up and writes every hit and its mirror
+// into its read's bucket: bfirst = bucket starts per read id (n_seq + 1), cur = fill cursors, out = the hit buckets.
 template <int PASS>
-__global__ void __launch_bounds__(PT_THREADS)
-k_win_tiles(const char *__restrict__ text, size_t len, unsigned *tile_ctr, LineTileState tstate, int min_span, int min_match, int bi_dir, WinTab tab,
-            const uint32_t *__restrict__ bfirst, uint32_t *cur, DHit *out, unsigned long long *ws)
-{
-	typedef cub::BlockScan<uint32_t, PT_THREADS> BS;
-	__shared__ __align__(16) char s_text[PT_TILE + PT_OVER + 16];
-	__shared__ uint16_t s_start[PT_LIST + 1];
-	__shared__ uint32_t s_vals[PT_THREADS / 32][11][32];
-	__shared__ typename BS::TempStorage s_scan;
-	__shared__ typename LinePrefixOp::TempStorage s_pref;
-	__shared__ unsigned long long s_first, s_tile, s_eol;
-	__shared__ uint32_t s_nl;
-	const uint32_t lane = threadIdx.x & 31;
-	if (threadIdx.x == 0) s_tile = atomicAdd(tile_ctr, 1u), s_nl = ~0u;
-	__syncthreads();
-	const uint64_t t = s_tile, b0 = t * PT_TILE, b1 = b0 + PT_TILE < len ? b0 + PT_TILE : len;
-	const uint64_t w_end = b1 + PT_OVER < len ? b1 + PT_OVER : len;           // staged bytes: [b0, w_end)
-	{
-		const uint32_t n16 = (uint32_t)((w_end - b0 + 15) >> 4);  // the tail word may reach past `len` but stays inside the (padded) window
-		for (uint32_t k = threadIdx.x; k < n16; k += PT_THREADS)
-			reinterpret_cast<uint4*>(s_text)[k] = __ldg(reinterpret_cast<const uint4*>(text + b0) + k);
-	}
-	__syncthreads();
-	const uint32_t my0 = threadIdx.x * 64, lim = (uint32_t)((b1 == len ? len - 1 : b1) - b0);
-	uint64_t bits = 0;
-	#pragma unroll
-	for (int k = 0; k < 4; ++k) bits |= (uint64_t)nl_bits_u4(reinterpret_cast<const uint4*>(s_text + my0)[k]) << (16 * k);
-	bits &= lim <= my0 ? 0ull : lim - my0 >= 64 ? ~0ull : (1ull << (lim - my0)) - 1;
-	const bool line0 = t == 0 && threadIdx.x == 0;            // the window's first line starts at its byte 0
-	uint32_t rank, n;
-	BS(s_scan).ExclusiveSum((uint32_t)__popcll(bits) + line0, rank, n);
-	for (uint32_t o = lim + threadIdx.x; o < (uint32_t)(w_end - b0); o += PT_THREADS)
-		if (s_text[o] == '\n' && b0 + o < len) { atomicMin(&s_nl, o); break; }
-	if (threadIdx.x < 32) {
-		if (t == 0) {
-			if (threadIdx.x == 0) tstate.SetInclusive(0, n), s_first = 0;
-		} else {
-			LinePrefixOp op(tstate, s_pref, ::cuda::std::plus<unsigned long long>(), (int)t);
-			const unsigned long long ex = op(n);
-			if (threadIdx.x == 0) s_first = ex;
-		}
-	}
-	__syncthreads();
-	const uint64_t first = ws[WS_LINE_IN] + s_first;          // global number of the tile's first line
-	if (threadIdx.x == 0 && b1 == len) ws[WS_LINE_OUT] = first + n;
-	if (n == 0) return;
-	uint64_t last_eol = s_nl != ~0u ? b0 + s_nl : w_end >= len ? len : ~0ull; // ~0: the tile's last line ends past the overhang
-	if (last_eol == ~0ull) {
-		if (threadIdx.x < 32) {
-			uint64_t e = len;
-			for (uint64_t p = w_end; p < len; p += 32 * 16) {
-				const uint64_t q = p + 16 * lane;
-				uint32_t m = 0;
-				for (uint32_t k = 0; k < 16 && q + k < len; ++k) m |= (uint32_t)(text[q + k] == '\n') << k;
-				const unsigned hit = __ballot_sync(0xffffffffu, m != 0);
-				if (hit) { e = __shfl_sync(0xffffffffu, q + __ffs(m) - 1, __ffs(hit) - 1); break; }
-			}
-			if (threadIdx.x == 0) s_eol = e;
-		}
-		__syncthreads();
-		last_eol = s_eol;
-	}
-	unsigned n_parsed = 0, n_pass = 0, n_bad = 0, n_emit = 0;
+struct WinParse {
+	WinTab tab;
+	unsigned long long *ws;
+	const uint32_t *bfirst;
+	uint32_t *cur;
+	DHit *out;
+	unsigned n_bad = 0, n_emit = 0;                           // (pass 2, per thread)
 	unsigned long long last11 = 0;                            // (1 + line) << 31 | bl of this thread's last line with an 11th field
-	for (uint32_t r0 = 0; r0 < n; r0 += PT_LIST) {
-		{
-			uint32_t r = rank;
-			uint64_t b = bits;
-			if (line0) { if (r == r0) s_start[0] = 0; ++r; }
-			for (; b && r <= r0 + PT_LIST; ++r, b &= b - 1)
-				if (r >= r0) s_start[r - r0] = (uint16_t)(my0 + __ffsll((long long)b));
+
+	__device__ __forceinline__ uint64_t line_base() const { return ws[WS_LINE_IN]; }
+	__device__ __forceinline__ void lines_end(uint64_t n) const { ws[WS_LINE_OUT] = n; }
+	__device__ __forceinline__ void cut() const {}            // (never: a window is launched with all of its bytes present)
+	__device__ __forceinline__ uint32_t *hits() const { return PASS == 1 ? tab.t.hits : nullptr; }
+	__device__ __forceinline__ void line(const char *text, const char *base, uint64_t s, uint64_t i, const PLine &r, bool stored, int bi_dir, uint32_t &sq, uint32_t &st)
+	{
+		if (PASS == 2 && r.nf >= 11) last11 = (i + 1) << 31 | (r.bl & 0x7fffffffu);
+		if (!stored) return;
+		if (PASS == 1) {
+			sq = win_insert(tab, text, base + s, r.qnl, s, 2 * i, r.ql, ws);
+			st = win_insert(tab, text, base + s + r.tdelta, r.tnl, s + r.tdelta, 2 * i + 1, r.tl, ws);
+			return;
 		}
-		__syncthreads();
-		const uint32_t cnt = n - r0 < PT_LIST ? n - r0 : PT_LIST;
-		for (uint32_t j0 = 0; j0 < cnt; j0 += PT_THREADS) {
-			const uint32_t j = j0 + threadIdx.x;
-			const uint64_t i = first + r0 + j;
-			uint32_t sq = NOSLOT, st = 0;
-			if (j < cnt) {
-				const uint64_t s = b0 + s_start[j];
-				uint64_t eol = r0 + j + 1 < n ? b0 + s_start[j + 1] - 1 : last_eol;
-				const char *base = eol <= w_end ? s_text - b0 : text; // base + window offset = address of that byte
-				if (eol - s > 1 && base[eol - 1] == '\r') --eol;
-				PLine r;
-				parse_line(base + s, base + eol, r, &s_vals[threadIdx.x >> 5][0][lane]);
-				if (r.nf >= 10) {
-					++n_parsed;
-					if (PASS == 2 && r.nf >= 11) last11 = (i + 1) << 31 | (r.bl & 0x7fffffffu);
-					if (!(r.qe - r.qs < (uint32_t)min_span || r.te - r.ts < (uint32_t)min_span || (int)(r.ml_rev & 0x7fffffffu) < min_match)) {
-						++n_pass;
-						if (PASS == 1) {
-							sq = win_insert(tab, text, base + s, r.qnl, s, 2 * i, r.ql, ws);
-							st = win_insert(tab, text, base + s + r.tdelta, r.tnl, s + r.tdelta, 2 * i + 1, r.tl, ws);
-						} else {
-							sq = win_find(tab, base + s, r.qnl), st = win_find(tab, base + s + r.tdelta, r.tnl);
-							if (sq == NOSLOT || st == NOSLOT) ++n_bad;  // a name pass 1 did not see: the source delivered other bytes
-							else {
-								const uint32_t qid = tab.t.id[sq], tid = tab.t.id[st], ord = (uint32_t)(2 * i);
-								const uint32_t bl = r.nf >= 11 ? r.bl & 0x7fffffffu : win_prev_bl(text, s, ws[WS_BL_IN]);
-								uint32_t at = atomicAdd(&cur[qid], 1u);
-								if (at < bfirst[qid + 1] - bfirst[qid]) {
-									uint4 *o = reinterpret_cast<uint4*>(out + bfirst[qid] + at);
-									o[0] = make_uint4(r.qs, ord, r.qe, tid);
-									o[1] = make_uint4(r.ts, r.te, r.ml_rev, bl);
-									++n_emit;
-								} else ++n_bad;                            // more hits than pass 1 counted for the read
-								if (bi_dir && qid != tid) { // the same overlap seen from the target (hit.c:92-98)
-									at = atomicAdd(&cur[tid], 1u);
-									if (at < bfirst[tid + 1] - bfirst[tid]) {
-										uint4 *o = reinterpret_cast<uint4*>(out + bfirst[tid] + at);
-										o[0] = make_uint4(r.ts, ord + 1, r.te, qid);
-										o[1] = make_uint4(r.qs, r.qe, r.ml_rev, bl);
-										++n_emit;
-									} else ++n_bad;
-								}
-							}
-						}
-					}
-				}
-			}
-			if (PASS == 1) { // consecutive lines often share their query read: one add per distinct slot of the warp
-				const unsigned grp = __match_any_sync(0xffffffffu, sq);
-				if (sq != NOSLOT && lane == (uint32_t)__ffs(grp) - 1) atomicAdd(&tab.t.hits[sq], (uint32_t)__popc(grp));
-				if (sq != NOSLOT && bi_dir && st != sq) atomicAdd(&tab.t.hits[st], 1u);
-			}
+		const uint32_t fq = win_find(tab, base + s, r.qnl), ft = win_find(tab, base + s + r.tdelta, r.tnl);
+		if (fq == NOSLOT || ft == NOSLOT) { ++n_bad; return; }    // a name pass 1 did not see: the source delivered other bytes
+		const uint32_t qid = tab.t.id[fq], tid = tab.t.id[ft], ord = (uint32_t)(2 * i);
+		const uint32_t bl = r.nf >= 11 ? r.bl & 0x7fffffffu : win_prev_bl(text, s, ws[WS_BL_IN]);
+		uint32_t at = atomicAdd(&cur[qid], 1u);
+		if (at < bfirst[qid + 1] - bfirst[qid]) {
+			uint4 *o = reinterpret_cast<uint4*>(out + bfirst[qid] + at);
+			o[0] = make_uint4(r.qs, ord, r.qe, tid);
+			o[1] = make_uint4(r.ts, r.te, r.ml_rev, bl);
+			++n_emit;
+		} else ++n_bad;                                          // more hits than pass 1 counted for the read
+		if (bi_dir && qid != tid) { // the same overlap seen from the target (hit.c:92-98)
+			at = atomicAdd(&cur[tid], 1u);
+			if (at < bfirst[tid + 1] - bfirst[tid]) {
+				uint4 *o = reinterpret_cast<uint4*>(out + bfirst[tid] + at);
+				o[0] = make_uint4(r.ts, ord + 1, r.te, qid);
+				o[1] = make_uint4(r.qs, r.qe, r.ml_rev, bl);
+				++n_emit;
+			} else ++n_bad;
 		}
-		__syncthreads(); // the list is rewritten by the next round
 	}
-	n_parsed = __reduce_add_sync(0xffffffffu, n_parsed), n_pass = __reduce_add_sync(0xffffffffu, n_pass);
-	if (PASS == 2) {
-		n_bad = __reduce_add_sync(0xffffffffu, n_bad), n_emit = __reduce_add_sync(0xffffffffu, n_emit);
-		#pragma unroll
-		for (int o = 16; o; o >>= 1) { const unsigned long long y = __shfl_xor_sync(0xffffffffu, last11, o); last11 = y > last11 ? y : last11; }
+	__device__ __forceinline__ void flush(uint32_t lane, unsigned n_parsed, unsigned n_pass)
+	{
+		if (PASS == 2) {
+			n_bad = __reduce_add_sync(0xffffffffu, n_bad), n_emit = __reduce_add_sync(0xffffffffu, n_emit);
+			#pragma unroll
+			for (int o = 16; o; o >>= 1) { const unsigned long long y = __shfl_xor_sync(0xffffffffu, last11, o); last11 = y > last11 ? y : last11; }
+		}
+		if (lane == 0) {
+			if (n_parsed) atomicAdd(ws + WS_PARSED, (unsigned long long)n_parsed);
+			if (n_pass) atomicAdd(ws + WS_STORED, (unsigned long long)n_pass);
+			if (n_bad) atomicAdd(ws + WS_BAD, (unsigned long long)n_bad);
+			if (n_emit) atomicAdd(ws + WS_EMITTED, (unsigned long long)n_emit);
+			if (last11) atomicMax(ws + WS_BL_OUT, last11);
+		}
 	}
-	if (lane == 0) {
-		if (n_parsed) atomicAdd(ws + WS_PARSED, (unsigned long long)n_parsed);
-		if (n_pass) atomicAdd(ws + WS_STORED, (unsigned long long)n_pass);
-		if (n_bad) atomicAdd(ws + WS_BAD, (unsigned long long)n_bad);
-		if (n_emit) atomicAdd(ws + WS_EMITTED, (unsigned long long)n_emit);
-		if (last11) atomicMax(ws + WS_BL_OUT, last11);
-	}
-}
+};
 
 // ids and per-read counts from the dictionary of pass 1 (k_dict_rank without a text to read back from: the witness is in the
 // name store and first carries the length column)
@@ -1698,6 +1637,28 @@ struct WinRun {
 		ts = tiles_alloc(d, w / PT_TILE + 1, &ts_mem);
 		cap = w;
 	}
+	// witness offsets count through the name store, then through the window (WinTab)
+	void check_offsets(uint64_t store_cap) const
+	{
+		if (store_cap + cap >= (1ull << NT_OFF_BITS) - 1) { fprintf(stderr, "[E::miniasm_b200] more than 2^37 bytes of read names and window\n"); exit(73); }
+	}
+	// a line longer than the window: the windows double, keeping the first `keep` bytes of window b
+	void grow(int b, size_t keep, uint64_t store_cap)
+	{
+		resize(2 * cap, b, keep);
+		check_offsets(store_cap);
+	}
+	// parses the first `cut` bytes of window b, once they have landed (stream order), and hands its line count and bl on to the next window
+	template <int PASS>
+	void launch(int b, size_t cut, int min_span, int min_match, int bi_dir, const WinParse<PASS> &pol)
+	{
+		const uint64_t n_tile = (cut + PT_TILE - 1) / PT_TILE;
+		tiles_reset(d, ts, n_tile);
+		MAB_CUDA(cudaMemsetAsync(ctr, 0, 4, d.stream));
+		MAB_LAUNCH(d, k_parse_tiles<WinParse<PASS>>, (unsigned)n_tile, PT_THREADS, 0, dev[b], cut, cut, 0, ~0ull, ctr, ts, min_span, min_match, bi_dir, pol);
+		MAB_CUDA(cudaMemcpyAsync(ws + WS_LINE_IN, ws + WS_LINE_OUT, 16, cudaMemcpyDeviceToDevice, d.stream));
+		MAB_CUDA(cudaEventRecord(parsed[b], d.stream));
+	}
 };
 
 // One pass over the source: false when it cannot be rewound.  *n_bytes = bytes delivered.
@@ -1706,8 +1667,9 @@ static bool win_pass(WinRun &w, int min_span, int min_match, int bi_dir, const W
 {
 	MabDev &d = w.d;
 	if (w.src.rewind(w.src.ud) != 0) return false;
-	if (tab.store_cap + w.cap >= (1ull << NT_OFF_BITS) - 1) { fprintf(stderr, "[E::miniasm_b200] more than 2^37 bytes of read names and window\n"); exit(73); }
+	w.check_offsets(tab.store_cap);
 	MAB_CUDA(cudaMemsetAsync(w.ws, 0, WS_N * 8, d.stream));
+	const WinParse<PASS> pol{tab, w.ws, bfirst, cur, out};
 	cudaEvent_t ready;
 	MAB_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
 	MAB_CUDA(cudaEventRecord(ready, d.stream));                 // the copies may not overtake whatever still uses the windows' memory on the main stream
@@ -1749,17 +1711,11 @@ static bool win_pass(WinRun &w, int min_span, int min_match, int bi_dir, const W
 					}
 					if (nl) { cut = (size_t)nl; break; }
 				}
-				w.resize(2 * w.cap, b, have);                       // a line longer than the window: the windows grow
-				if (tab.store_cap + w.cap >= (1ull << NT_OFF_BITS) - 1) { fprintf(stderr, "[E::miniasm_b200] more than 2^37 bytes of read names and window\n"); exit(73); }
+				w.grow(b, have, tab.store_cap);                     // a line longer than the window
 			}
 			tail_at = cut, n_tail = have - cut;
 			if (cut == 0) break;
-			const uint64_t n_tile = (cut + PT_TILE - 1) / PT_TILE;
-			tiles_reset(d, w.ts, n_tile);
-			MAB_CUDA(cudaMemsetAsync(w.ctr, 0, 4, d.stream));
-			MAB_LAUNCH(d, k_win_tiles<PASS>, (unsigned)n_tile, PT_THREADS, 0, w.dev[b], cut, w.ctr, w.ts, min_span, min_match, bi_dir, tab, bfirst, cur, out, w.ws);
-			MAB_CUDA(cudaMemcpyAsync(w.ws + WS_LINE_IN, w.ws + WS_LINE_OUT, 16, cudaMemcpyDeviceToDevice, d.stream));
-			MAB_CUDA(cudaEventRecord(w.parsed[b], d.stream));
+			w.launch(b, cut, min_span, min_match, bi_dir, pol);
 		}
 	}
 	for (int b = 0; !eof; b ^= 1) {
@@ -1775,8 +1731,7 @@ static bool win_pass(WinRun &w, int min_span, int min_match, int bi_dir, const W
 			if (eof) { cut = have; break; }
 			const char *nl = (const char*)memrchr(w.host[b], '\n', have);
 			if (nl) { cut = (size_t)(nl - w.host[b]) + 1; break; }
-			w.resize(2 * w.cap, b, have);                       // a line longer than the window: the windows grow
-			if (tab.store_cap + w.cap >= (1ull << NT_OFF_BITS) - 1) { fprintf(stderr, "[E::miniasm_b200] more than 2^37 bytes of read names and window\n"); exit(73); }
+			w.grow(b, have, tab.store_cap);                     // a line longer than the window
 		}
 		tail = w.host[b] + cut, n_tail = have - cut;
 		if (cut == 0) break;                                    // (the end of the source, nothing left)
@@ -1784,12 +1739,7 @@ static bool win_pass(WinRun &w, int min_span, int min_match, int bi_dir, const W
 		MAB_CUDA(cudaMemcpyAsync(w.dev[b], w.host[b], cut, cudaMemcpyHostToDevice, d.copy_stream));
 		MAB_CUDA(cudaEventRecord(w.copied[b], d.copy_stream));
 		MAB_CUDA(cudaStreamWaitEvent(d.stream, w.copied[b], 0));
-		const uint64_t n_tile = (cut + PT_TILE - 1) / PT_TILE;
-		tiles_reset(d, w.ts, n_tile);
-		MAB_CUDA(cudaMemsetAsync(w.ctr, 0, 4, d.stream));
-		MAB_LAUNCH(d, k_win_tiles<PASS>, (unsigned)n_tile, PT_THREADS, 0, w.dev[b], cut, w.ctr, w.ts, min_span, min_match, bi_dir, tab, bfirst, cur, out, w.ws);
-		MAB_CUDA(cudaMemcpyAsync(w.ws + WS_LINE_IN, w.ws + WS_LINE_OUT, 16, cudaMemcpyDeviceToDevice, d.stream));
-		MAB_CUDA(cudaEventRecord(w.parsed[b], d.stream));
+		w.launch(b, cut, min_span, min_match, bi_dir, pol);
 	}
 	d.sync();
 	MAB_CUDA(cudaEventDestroy(ready));
@@ -1800,9 +1750,7 @@ static bool win_pass(WinRun &w, int min_span, int min_match, int bi_dir, const W
 bool ingest_paf_windowed(MabDev &d, const TextSource &src, size_t window_bytes, size_t size_hint, int min_span, int min_match, int bi_dir,
                          DHits &h, DNames &names, char **name_text_out, IngestStats &st)
 {
-	memset(&st, 0, sizeof(st));
-	names = DNames();
-	h.n = 0, h.n_seq = 0;
+	ingest_open(0, h, names, st);
 	*name_text_out = nullptr;
 	d.trace("ingest:begin");
 	if (window_bytes < (64u << 10)) window_bytes = 64u << 10;
@@ -1835,52 +1783,11 @@ bool ingest_paf_windowed(MabDev &d, const TextSource &src, size_t window_bytes, 
 		dh_reserve(d, h, 1);
 		return true;
 	}
-	// ids = rank of the first occurrence; the hit counts of the slots become those of the reads
-	uint64_t *slots = mab_alloc<uint64_t>(d, cap);
-	uint32_t n_seq;
-	{
-		cub::CountingInputIterator<uint64_t> pos(0);
-		SlotUsed used{tab.t.first};
-		size_t tb = 0;
-		unsigned long long *d_n = d.d_scal + SC_NSEL;
-		cub::DeviceSelect::If(nullptr, tb, pos, slots, d_n, (int64_t)cap, used, d.stream);
-		void *tmp = d.tmp(tb);
-		cub::DeviceSelect::If(tmp, tb, pos, slots, d_n, (int64_t)cap, used, d.stream);
-		++d.n_lib;
-		const uint64_t n = d.get_scal(SC_NSEL);
-		if (n >= (1ull << 31)) { fprintf(stderr, "[E::miniasm_b200] more than 2^31 reads\n"); exit(73); }
-		n_seq = (uint32_t)n;
-	}
-	names.n_seq = n_seq;
-	names.off = mab_alloc<uint64_t>(d, n_seq); names.nlen = mab_alloc<uint32_t>(d, n_seq); names.slen = mab_alloc<uint32_t>(d, n_seq);
-	uint32_t *read_cnt = mab_alloc<uint32_t>(d, (size_t)n_seq + 1), *first = mab_alloc<uint32_t>(d, (size_t)n_seq + 1);
-	MAB_CUDA(cudaMemsetAsync(read_cnt + n_seq, 0, 4, d.stream));
-	if (n_seq) {
-		unsigned long long *fa = (unsigned long long*)mab_alloc<uint64_t>(d, n_seq), *fb = (unsigned long long*)mab_alloc<uint64_t>(d, n_seq);
-		uint64_t *sb = mab_alloc<uint64_t>(d, n_seq);
-		MAB_LAUNCH(d, k_dict_pairs, mab_grid(n_seq, 256), 256, 0, slots, n_seq, tab.t, fa);
-		cub::DoubleBuffer<unsigned long long> dk(fa, fb);
-		cub::DoubleBuffer<uint64_t> dv(slots, sb);
-		size_t tb = 0;
-		cub::DeviceRadixSort::SortPairs(nullptr, tb, dk, dv, (int)n_seq, 32, 64, d.stream);   // by the occurrence number, the high half
-		void *tmp = d.tmp(tb);
-		cub::DeviceRadixSort::SortPairs(tmp, tb, dk, dv, (int)n_seq, 32, 64, d.stream);
-		++d.n_lib;
-		d.zero_scal(SC_AUX, 1);
-		MAB_LAUNCH(d, k_win_rank, mab_grid(n_seq, 256), 256, 0, dk.Current(), dv.Current(), n_seq, tab, names.off, names.nlen, names.slen, d.d_scal + SC_AUX, read_cnt);
-		st.tot_len = d.get_scal(SC_AUX);
-		d.free(fa); d.free(fb); d.free(sb);
-	}
-	d.free(slots);
-	d.trace("ingest:rank_ids");
-	dh_bucket_first(d, read_cnt, n_seq, first);
-	MAB_CUDA(cudaMemsetAsync(read_cnt, 0, (size_t)n_seq * 4, d.stream)); // the counts become the buckets' fill cursors
-	uint32_t n_hits;
-	MAB_CUDA(cudaMemcpyAsync(&n_hits, first + n_seq, 4, cudaMemcpyDeviceToHost, d.stream));
-	d.sync();
-	dh_reserve(d, h, n_hits ? n_hits : 1);
-	h.n = n_hits, h.n_seq = n_seq;
-	st.n_hits = n_hits, st.n_seq = n_seq;
+	// ids = rank of the first occurrence (the high half of first[slot]); the hit counts of the slots become those of the reads
+	uint32_t *read_cnt, *first;
+	rank_reads(d, tab.t, cap, 32, 64, [&](const unsigned long long *fs, const uint64_t *ss, uint32_t n, unsigned long long *tot, uint32_t *cnt) {
+		MAB_LAUNCH(d, k_win_rank, mab_grid(n, 256), 256, 0, fs, ss, n, tab, names.off, names.nlen, names.slen, tot, cnt);
+	}, h, names, st, read_cnt, first);
 	// pass 2: every hit straight into its read's bucket of h.a2
 	uint64_t n_bytes2 = 0;
 	const bool ok2 = win_pass<2>(w, min_span, min_match, bi_dir, tab, first, read_cnt, h.a2, &n_bytes2);
@@ -1892,9 +1799,9 @@ bool ingest_paf_windowed(MabDev &d, const TextSource &src, size_t window_bytes, 
 		h.n = 0, h.n_seq = 0;
 		return false;
 	}
-	if (n_bytes2 != n_bytes || ws[WS_LINE_IN] != n_lines || ws[WS_PARSED] != st.n_parsed || ws[WS_STORED] != n_stored || ws[WS_BAD] || ws[WS_EMITTED] != n_hits) {
+	if (n_bytes2 != n_bytes || ws[WS_LINE_IN] != n_lines || ws[WS_PARSED] != st.n_parsed || ws[WS_STORED] != n_stored || ws[WS_BAD] || ws[WS_EMITTED] != st.n_hits) {
 		fprintf(stderr, "[E::miniasm_b200] the PAF source delivered a different text after rewinding: %llu bytes, %llu lines, %llu hits first, "
-		        "%llu bytes, %llu lines, %llu hits (%llu without a bucket) then\n", (unsigned long long)n_bytes, (unsigned long long)n_lines, (unsigned long long)n_hits,
+		        "%llu bytes, %llu lines, %llu hits (%llu without a bucket) then\n", (unsigned long long)n_bytes, (unsigned long long)n_lines, (unsigned long long)st.n_hits,
 		        (unsigned long long)n_bytes2, ws[WS_LINE_IN], ws[WS_EMITTED], ws[WS_BAD]);
 		exit(78);
 	}
